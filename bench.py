@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native LeetCUDA hot paths.
+"""bench.py — headline benchmark of the H100-native LeetCUDA hot paths.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Primary line (BASELINE.json configs[1]): HGEMM fp16 M=N=K=8192 through the reference-facing op
 `hgemm_mma_m16n8k16_mma2x4_warp4x4x2_stages_dsmem_swizzle` (NN layout).  One "step" = one GEMM
@@ -17,19 +17,25 @@ the fused rope / rms-norm steps around attention).
 * value      whole-job TFLOPS, inputs resident in HBM, CUDA-event timed, max over ranks
 * e2e        same metric through the public host-buffer call: H2D of the inputs and D2H of the
              result inside the timed region, every step
-* roofline   tensor-bound: algorithmic FLOPs / measured kernel time vs MEASURED_PEAKS.json
+* roofline   tensor-bound: algorithmic FLOPs / measured kernel time vs MEASURED_PEAKS.json (else the H100 SXM data sheet)
 * cpu_baseline  torch.matmul / SDPA on the host cores (north_star's CPU path), bounded sample
 
 N > 1 (torchrun, one rank per GPU): BASELINE configs[4], HGEMM 16384^3 row-sharded over the ranks
 (strong scaling, SURVEY §8e) — rank r owns 16384/N rows of A and C, B replicated, and every rank
 ends with the full [16384, 16384] C: the GEMM epilogue pushes each finished box of C to all peers
-with TMA stores over NVLink (fused all-gather, leetcuda_b200/dist.py), closed by a symmetric-memory
+with stores over NVLink (fused all-gather, leetcuda_b200/dist.py), closed by a symmetric-memory
 barrier.  The same run also times the stated baseline, GEMM + ncclAllGather (`nccl_baseline`).
 B200_DIST_TRANSPORT=nccl makes that baseline the headline transport.  The N = 1 line carries the
 single-GPU 16384^3 figure (`strong_scaling_n1`) the N > 1 values are to be compared with.
 
 --impl reference times the reference's CPU path (torch.matmul on the host cores, all threads) on
 the same workload as this arm at the same N; rank 0 only.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step of each row computed (HGEMM C, the attention
+outputs O, the TF32 SGEMM C, merge_attn_states output and LSE, rope, rms_norm, rope of q and k, the fused and unfused
+RMS-norm attention outputs) as DIR/<name>.npy in float32: a fixed, seeded sample of 1 Mi elements of each (4 MiB,
+13 files).  The
+inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -56,10 +62,10 @@ def line_config(world: int, transport: str) -> dict:
     if world == 1:
         return {"workload": "hgemm_nn_8192x8192x8192_fp16", "op": OP, "accumulate": "fp32",
                 "parallelism": "single GPU",
-                "l2": "operands rotate over 3 sets, each > 126 MB L2: no flush needed"}
+                "l2": "operands rotate over 3 sets, each > 50 MB L2: no flush needed"}
     return {"workload": f"hgemm_nn_16384x16384x16384_fp16_rowsharded_x{world}_allgatherC", "op": OP,
             "accumulate": "fp32", "parallelism": f"row-shard x{world}, transport {transport}",
-            "l2": "operands rotate over 2 sets, each > 126 MB L2: no flush needed"}
+            "l2": "operands rotate over 2 sets, each > 50 MB L2: no flush needed"}
 
 
 def line_metric(world: int) -> str:
@@ -74,7 +80,7 @@ def measured_peaks():
             return float(d["bf16_tflops"]), float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst)"
         except Exception:
             pass
-    return 1590.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense fp16, HBM3; 700 W card)"
 
 
 class ClockSampler:
@@ -145,6 +151,21 @@ class ClockSampler:
         s = sorted(self.samples)
         return {"sm_mhz": (s[len(s) // 2] if s else None), "sm_max_mhz": self.max_mhz,
                 "reasons": sorted(self.reasons), "samples": len(s)}
+
+
+def dump_output(dump_dir, name, t, n=1 << 20):
+    """DIR/<name>.npy: float32 values of tensor t at n fixed, seeded positions (all of it if smaller)."""
+    if dump_dir is None:
+        return
+    import numpy as np
+    import torch
+    flat = t.reshape(-1)
+    if flat.numel() > n:
+        idx = np.sort(np.random.default_rng(0).integers(0, flat.numel(), n))
+        flat = flat[torch.from_numpy(idx).to(flat.device)]
+    out = Path(dump_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    np.save(out / f"{name}.npy", flat.float().cpu().numpy())
 
 
 def settle(seconds: float = 0.75):
@@ -223,39 +244,56 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
-def cpu_baselines():
-    """torch.matmul / SDPA on the host cores, bounded samples (rank 0, N=1 only)."""
+def cpu_baselines(budget: float = 15.0):
+    """torch.matmul / SDPA on the host cores (rank 0, N=1 only).  Like run_reference, each problem is timed whole when
+    that fits the time budget and otherwise on the largest slab of it that does (rows of A; query rows of the attention,
+    whole heads once one head fits), sized from an untimed probe: fp16 on a host CPU without a native fp16 path runs
+    at well under 1 GFLOP/s.  The `sample` field says which."""
     import torch
     import torch.nn.functional as F
     cores = torch.get_num_threads()
     torch.manual_seed(0)
-    a = torch.randn(S, S, dtype=torch.half)
     b = torch.randn(S, S, dtype=torch.half)
-    torch.matmul(a[:512], b)
+    probe = torch.randn(8, S, dtype=torch.half)
+    torch.matmul(probe, b)                                             # first touch of b, thread pool start
     t0 = time.perf_counter()
-    torch.matmul(a, b)                       # the whole 8192^3 problem, once (about a second)
+    torch.matmul(probe, b)                                             # probe: 8 rows
+    per_row = (time.perf_counter() - t0) / 8
+    rows = max(8, min(S, int(budget / per_row) // 8 * 8))
+    a = torch.randn(rows, S, dtype=torch.half)
+    t0 = time.perf_counter()
+    torch.matmul(a, b)
     dt = time.perf_counter() - t0
-    gemm = {"value": 2.0 * S * S * S / dt / 1e12, "unit": "TFLOPS", "cores": cores, "kind": "reference",
-            "sample": f"torch.matmul fp16 on host cores, the whole 8192^3 problem once ({dt:.1f} s)"}
+    what = "the whole 8192^3 problem" if rows == S else f"a {rows}-row slab of the 8192^3 problem"
+    gemm = {"value": 2.0 * rows * S * S / dt / 1e12, "unit": "TFLOPS", "cores": cores, "kind": "reference",
+            "sample": f"torch.matmul fp16 on host cores, {what} once ({dt:.1f} s)"}
+    del a, b
 
-    def sdpa_sample(B, H, N, D, max_reps, label):
-        q, k, v = (torch.randn(B, H, N, D, dtype=torch.half) for _ in range(3))
-        F.scaled_dot_product_attention(q[:, :1], k[:, :1], v[:, :1])
-        reps, dt, t0 = 0, 0.0, time.perf_counter()
-        while reps < max_reps and dt < 10.0:
-            F.scaled_dot_product_attention(q, k, v)
-            reps += 1
-            dt = time.perf_counter() - t0
-        return {"value": 4.0 * reps * B * H * N * N * D / dt / 1e12, "unit": "TFLOPS", "cores": cores, "kind": "reference",
-                "sample": f"F.scaled_dot_product_attention fp16 on host cores, {reps} x (B{B} H{H} N{N} D{D}) of {label} ({dt:.1f} s)"}
+    def sdpa_sample(B, H, N, D, label):
+        k, v = (torch.randn(1, 1, N, D, dtype=torch.half) for _ in range(2))
+        probe = torch.randn(1, 1, 16, D, dtype=torch.half)
+        F.scaled_dot_product_attention(probe, k, v)
+        t0 = time.perf_counter()
+        F.scaled_dot_product_attention(probe, k, v)                    # probe: 16 query rows
+        per_q = (time.perf_counter() - t0) / 16
+        nq = max(16, min(B * H * N, int(budget / per_q)))
+        heads = max(1, nq // N) if nq >= N else 1
+        qn = N if nq >= N else nq
+        q, k, v = (torch.randn(1, heads, n, D, dtype=torch.half) for n in (qn, N, N))
+        t0 = time.perf_counter()
+        F.scaled_dot_product_attention(q, k, v)
+        dt = time.perf_counter() - t0
+        what = (f"{heads} of the {B * H} (batch x head) units" if qn == N else f"{qn} query rows of one head")
+        return {"value": 4.0 * heads * qn * N * D / dt / 1e12, "unit": "TFLOPS", "cores": cores, "kind": "reference",
+                "sample": f"F.scaled_dot_product_attention fp16 on host cores, {what} of {label} ({dt:.1f} s)"}
 
-    attn = sdpa_sample(1, 8, FA[2], FA[3], 16, "B4 H32")      # 16 x (B1 H8) = the full problem
-    ffpa = sdpa_sample(1, 4, FF[2], FF[3], 8, "B2 H16")       # 8 x (B1 H4) = the full problem
+    attn = sdpa_sample(*FA, "B4 H32 N4096 D128")
+    ffpa = sdpa_sample(*FF, "B2 H16 N2048 D512")
     return gemm, attn, ffpa
 
 
 def attention_row(torch, dev, world, rank, args, sync, shape, op, op_name, metric, kernel, peak_tf, peak_src, traffic_file,
-                  host_op, want_e2e):
+                  host_op, want_e2e, dump_name=None):
     """One attention config: device-timed value, roofline, vendor SDPA, e2e through the host-buffer entry."""
     import torch.distributed as dist
     import torch.nn.functional as F
@@ -264,7 +302,7 @@ def attention_row(torch, dev, world, rank, args, sync, shape, op, op_name, metri
     assert (B * H) % world == 0
     Bw, Hw = (B, H) if world == 1 else (1, B * H // world)      # (batch x head) units are independent
     torch.manual_seed(4321 + rank)
-    nsets = 2 if 8 * Bw * Hw * N * D > 200e6 else 3              # rotate sets: > 126 MB L2 in flight
+    nsets = 2 if 8 * Bw * Hw * N * D > 200e6 else 3              # rotate sets: > 50 MB L2 in flight
     sets = [[torch.randn(Bw, Hw, N, D, device=dev, dtype=torch.half) for _ in range(3)] for _ in range(nsets)]
     outs = [torch.empty(Bw, Hw, N, D, device=dev, dtype=torch.half) for _ in range(nsets)]
 
@@ -280,6 +318,8 @@ def attention_row(torch, dev, world, rank, args, sync, shape, op, op_name, metri
     with ClockSampler(dev.index) as row_clk:
         fms = cuda_time_ms(fstep, args.steps, sync)
     launches = _capi.launch_count() - l1
+    if rank == 0 and dump_name:
+        dump_output(args.dump_outputs, dump_name, outs[(args.steps - 1) % nsets])
     tf = torch.tensor([fms], device=dev, dtype=torch.float64)
     if world > 1:
         dist.all_reduce(tf, op=dist.ReduceOp.MAX)
@@ -337,6 +377,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-secondary", action="store_true", help="skip the attention metrics and the next rows")
     ap.add_argument("--no-cpu", action="store_true", help="skip the CPU baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a fixed sample of what the last timed step of each row computed to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -374,7 +416,7 @@ def main():
         assert S16 % world == 0
         Mr, Nn, Kk = S16 // world, S16, S16
     torch.manual_seed(1234 + rank)
-    NSETS = 3 if world == 1 else 2  # rotate operand sets (each >> 126 MB L2): no L2-resident re-reads
+    NSETS = 3 if world == 1 else 2  # rotate operand sets (each >> 50 MB L2): no L2-resident re-reads
     As = [torch.randn(Mr, Kk, device=dev, dtype=torch.half) for _ in range(NSETS)]
     if world > 1:
         torch.manual_seed(99)  # B is replicated: same values on every rank
@@ -384,20 +426,23 @@ def main():
     sharded = bdist.RowShardedHgemm(Mr, Nn, Kk, world, rank, dev, transport=transport) if world > 1 else None
     Cs = [torch.empty(Mr, Nn, device=dev, dtype=torch.half) for _ in range(NSETS)] if world == 1 else None
 
+    last_c = [None]   # C of the latest step (the fused transport alternates two buffers)
+
     def step(i):
         j = i % NSETS
         if world == 1:
             op(As[j], Bs[j], Cs[j], 2, True, 2048)
+            last_c[0] = Cs[j]
         else:
-            sharded(As[j], Bs[j])
+            last_c[0] = sharded(As[j], Bs[j])
 
-    # N > 1, fused transport: the epilogue can push each finished box of C to every peer mapping (one TMA store per
-    # peer) or once through the NVLS multicast mapping.  Which is faster depends on N (egress bytes: (N-1)x vs 1x the
+    # N > 1, fused transport: the epilogue can store each finished value of C to every peer mapping or once through
+    # the NVLS multicast mapping.  Which is faster depends on N (egress bytes: (N-1)x vs 1x the
     # shard); pick by a short untimed trial, all ranks agreeing on the max-over-ranks time.  B200_FUSED_EPILOGUE pins it.
     epilogue = os.environ.get("B200_FUSED_EPILOGUE", "")
     if world > 1 and transport == "fused" and not epilogue:
         trial = {}
-        for mode in ("tma", "mc"):
+        for mode in ("peers", "mc"):
             os.environ["B200_FUSED_EPILOGUE"] = mode
             try:
                 for i in range(3):
@@ -420,6 +465,8 @@ def main():
     with ClockSampler(local) as clk:
         ms = cuda_time_ms(step, args.steps, sync)
     launches = _capi.launch_count() - l0
+    if rank == 0:
+        dump_output(args.dump_outputs, "hgemm_c", last_c[0])
     t = torch.tensor([ms], device=dev, dtype=torch.float64)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -443,16 +490,16 @@ def main():
     ach = flops_rank / (k_ms * 1e-3) / 1e12
     roofline = {"bound": "tensor", "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s",
                 "frac": ach / peak_tf, "traffic": None, "peak_source": peak_src,
-                "kernel": "hgemm_tcgen05_kernel<cta_group=2, NN>", "kernel_ms": k_ms,
+                "kernel": "hgemm_wgmma_kernel<128x256 tile, NN>", "kernel_ms": k_ms,
                 "algorithmic_flops": flops_rank, "algorithmic_bytes": 2 * (Mr * Kk + Kk * Nn + Mr * Nn)}
     if world > 1:
         gather = (world - 1) * Mr * Nn * 2
         roofline["fused_step"] = {
-            "nvlink_bytes_in_per_rank": gather, "nvlink_peak_gbs": 770.0,
-            "target_ms": max(flops_rank / (peak_tf * 1e12), gather / 770e9) * 1e3,
+            "nvlink_bytes_in_per_rank": gather, "nvlink_peak_gbs": 450.0,
+            "target_ms": max(flops_rank / (peak_tf * 1e12), gather / 450e9) * 1e3,
             "achieved_ms": ms_step, "compute_only_ms": k_ms,
             "epilogue": epilogue if transport == "fused" else None, "epilogue_trial_ms": trial if transport == "fused" else None,
-            "note": "target = slower of (FLOPs / measured GEMM peak) and (bytes received over NVLink / 770 GB/s)"}
+            "note": "target = slower of (FLOPs / measured GEMM peak) and (bytes received over NVLink / 450 GB/s, H100 NVLink 4 per direction)"}
         # the stated baseline in the same run: GEMM into the rank's slice, then one ncclAllGather of C
         try:
             base = sharded if transport == "nccl" else bdist.RowShardedHgemm(Mr, Nn, Kk, world, rank, dev, transport="nccl")
@@ -486,15 +533,15 @@ def main():
         secondary, nl = attention_row(
             torch, dev, world, rank, args, sync, FA, flash_attn.flash_attn_mma_stages_split_q_shared_qkv,
             "flash_attn_mma_stages_split_q_shared_qkv", "FA-2 fp16 TFLOPS @B4H32N4096D128 (matmul FLOPs 4BHN^2D)",
-            "attn_fwd_kernel<128> (two query tiles per CTA)", peak_tf, peak_src, "attn_traffic.json",
-            flash_attn.fmha_host, True)
+            "attn_fwd_kernel<128-column slab, 2 consumer warpgroups>", peak_tf, peak_src, "attn_traffic.json",
+            flash_attn.fmha_host, True, dump_name="attn_d128_o")
         launches += nl
         try:
             config4, nl = attention_row(
                 torch, dev, world, rank, args, sync, FF, ffpa_attn.ffpa_mma_acc_f32_L1,
                 "ffpa_mma_acc_f32_L1", "FFPA fp16 TFLOPS @B2H16N2048D512 (matmul FLOPs 4BHN^2D)",
-                "attn_pair_fwd_kernel (one query tile per CTA pair, cta_group::2)", peak_tf, peak_src,
-                "attn_pair_traffic.json", flash_attn.fmha_host, True)
+                "attn_fwd_kernel<256-column slabs, 1 consumer warpgroup>", peak_tf, peak_src,
+                "attn_pair_traffic.json", flash_attn.fmha_host, True, dump_name="ffpa_d512_o")
             launches += nl
         except Exception as e:
             config4 = {"error": f"{type(e).__name__}: {e}"}
@@ -503,8 +550,8 @@ def main():
             attn_d64, nl = attention_row(
                 torch, dev, world, rank, args, sync, (FA[0], FA[1], FA[2], 64), flash_attn.flash_attn_mma_stages_split_q_shared_qkv,
                 "flash_attn_mma_stages_split_q_shared_qkv", "FA-2 fp16 TFLOPS @B4H32N4096D64 (matmul FLOPs 4BHN^2D)",
-                "attn_fwd_kernel<64> (two query tiles per CTA, persistent grid)", peak_tf, peak_src, "attn_d64_traffic.json",
-                flash_attn.fmha_host, False)
+                "attn_fwd_kernel<64-column slab, 2 consumer warpgroups>", peak_tf, peak_src, "attn_d64_traffic.json",
+                flash_attn.fmha_host, False, dump_name="attn_d64_o")
             launches += nl
         except Exception as e:
             attn_d64 = {"error": f"{type(e).__name__}: {e}"}
@@ -625,6 +672,7 @@ def row_sgemm_tf32(torch, dev, args, peak_tf, peak_hbm, peak_src):
     # the reference op: TF32 rounding of a and b in place + GEMM (3 launches of ours per step)
     op_ms = cuda_time_ms(lambda i: SG.sgemm_wmma_m16n16k8_mma4x2_warp2x4_stages(
         sa[i % 2], sb[i % 2], sc[i % 2], 2, False, 1), args.steps, lambda: torch.cuda.synchronize()) / args.steps
+    dump_output(args.dump_outputs, "sgemm_tf32_c", sc[(args.steps - 1) % 2])
     # the GEMM kernel alone (operands already TF32-exact after the calls above)
     k_ms = cuda_time_ms(lambda i: SG.sgemm_tf32(sa[i % 2], sb[i % 2], sc[i % 2], round_inputs=False),
                         args.steps, lambda: torch.cuda.synchronize()) / args.steps
@@ -639,18 +687,18 @@ def row_sgemm_tf32(torch, dev, args, peak_tf, peak_hbm, peak_src):
                 for _ in range(10))
     torch.backends.cuda.matmul.allow_tf32 = prev
     ach = gfl / (k_ms * 1e-3) / 1e12
-    tf32_nominal = 1125.0     # half the dense bf16 figure of B200_PROFILING.md (2250): a NOMINAL denominator
+    tf32_nominal = 495.0      # dense TF32 of the H100 SXM data sheet: a NOMINAL denominator
     return {
         "metric": "SGEMM TF32 TFLOPS @8192^3 (reference op: round a,b to TF32 in place + GEMM)",
         "value": gfl / (op_ms * 1e-3) / 1e12, "unit": "TFLOPS", "ms_per_step": op_ms,
         "config": {"workload": "sgemm_nn_8192x8192x8192_fp32_tf32", "op": "sgemm_wmma_m16n16k8_mma4x2_warp2x4_stages"},
         "roofline": {"bound": "tensor", "achieved": ach, "peak": tf32_nominal, "unit": "TFLOP/s",
                      "frac": ach / tf32_nominal, "traffic": None,
-                     "peak_source": "NOMINAL dense TF32 (datasheet bf16 / 2; MEASURED_PEAKS.json has no TF32 entry) — "
+                     "peak_source": "NOMINAL dense TF32 (H100 SXM data sheet; MEASURED_PEAKS.json has no TF32 entry) — "
                                     "see measured_vendor_burst for the in-run cuBLAS TF32 figure",
                      "measured_vendor_burst": gfl / (burst * 1e-3) / 1e12,
                      "frac_of_measured_vendor_burst": ach / (gfl / (burst * 1e-3) / 1e12),
-                     "kernel": "hgemm_tcgen05_macro_kernel<NN, tf32> (512x256 per CTA pair)", "kernel_ms": k_ms,
+                     "kernel": "tf32_transpose_kernel + hgemm_wgmma_kernel<tf32, TN>", "kernel_ms": k_ms,
                      "algorithmic_bytes": 3 * 4 * Sg * Sg},
         "vendor": {"impl": "cuBLAS TF32 via torch.matmul (allow_tf32), back to back", "tflops": gfl / (v_ms * 1e-3) / 1e12},
     }
@@ -670,6 +718,8 @@ def row_merge(torch, dev, args, peak_tf, peak_hbm, peak_src):
         MA.merge_attn_states_cuda(mo[i % 2], mp[i % 2], mpl, ms[i % 2], msl, mol)
     m_ms = cuda_time_ms(lambda i: MA.merge_attn_states_cuda(mo[i % 2], mp[i % 2], mpl, ms[i % 2], msl, mol),
                         args.steps, lambda: torch.cuda.synchronize()) / args.steps
+    dump_output(args.dump_outputs, "merge_out", mo[(args.steps - 1) % 2])
+    dump_output(args.dump_outputs, "merge_lse", mol)
     m_bytes = Tm * Hm * (3 * Dm * 2 + 12)
     m_gbs = m_bytes / (m_ms * 1e-3) / 1e9
     row = {
@@ -692,7 +742,8 @@ def row_merge(torch, dev, args, peak_tf, peak_hbm, peak_src):
 def row_rope_rmsnorm(torch, dev, args, peak_tf, peak_hbm, peak_src):
     """§8f-4: the element-wise steps around attention (rope on q/k, rms-norm), HBM-bound."""
     from leetcuda_b200 import fused_ops as FO
-    return FO.bench_rows(torch, dev, args.steps, peak_hbm, peak_src, cuda_time_ms)
+    return FO.bench_rows(torch, dev, args.steps, peak_hbm, peak_src, cuda_time_ms,
+                         dump=lambda name, t: dump_output(args.dump_outputs, name, t))
 
 
 if __name__ == "__main__":

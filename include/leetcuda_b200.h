@@ -1,4 +1,4 @@
-/* leetcuda_b200.h — C ABI of the B200-native (sm_100a) replacement for LeetCUDA's
+/* leetcuda_b200.h — C ABI of the H100-native (sm_90a) replacement for LeetCUDA's
  * two dense-contraction hot paths.  Plain pointers and sizes only: no torch
  * types cross this boundary.  All device pointers must live on the CUDA device
  * that is current on the calling thread; `stream` is a cudaStream_t (NULL = the
@@ -40,7 +40,7 @@ const char* b200_last_error(void);
  * threads).  Used by bench.py to report `gpu_launches`. */
 uint64_t b200_launch_count(void);
 
-/* C[M,N] = A[M,K] x B, fp16 in / fp16 out, fp32 accumulation in TMEM.
+/* C[M,N] = A[M,K] x B, fp16 in / fp16 out, fp32 accumulation (wgmma, registers).
  *
  * Replaces every `void hgemm_*(torch::Tensor a, torch::Tensor b, torch::Tensor c
  * [, int stages, bool swizzle, int swizzle_stride])` bound in the reference's
@@ -59,21 +59,17 @@ int b200_hgemm_f16(const void* a, const void* b, void* c, int M, int N, int K, i
                    void* stream);
 
 /* Same as b200_hgemm_f16 with explicit tuning/debug knobs (0 = default):
- *   cta_group  1 | 2      tcgen05 cta_group (2 = CTA pair, 256x256 tile)
- *              3          CTA pair, 512x256 macro tile (two accumulators sharing B); 30..33 = the
- *                         same with accumulator 1 trailing accumulator 0 by 0|1|2 k-blocks
+ *   cta_group  1 | 2      output tile: 1 = 128x128, 2 = 128x256 (other values: B200_EINVAL)
  *   group_m    >0         m-tiles per rasterisation group
  *   max_ctas   >0         cap on the persistent grid
- *   b_lbo,b_sbo,b_kstep   UMMA descriptor byte offsets of the MN-major B operand; the top byte of
- *                         b_lbo carries two more debug overrides: bits [28,32) the UMMA layout type of
- *                         that descriptor, bits [24,28) the CUtensorMapSwizzle of the B tensor map
+ *   b_lbo,b_sbo,b_kstep   wgmma descriptor byte offsets of the MN-major B operand (fp16 [K,N] layout)
  */
 int b200_hgemm_f16_ex(const void* a, const void* b, void* c, int M, int N, int K, int b_layout,
                       int cta_group, int group_m, int max_ctas, uint32_t b_lbo, uint32_t b_sbo,
                       uint32_t b_kstep, void* stream);
 
 /* Reference-accumulation parity mode: same as b200_hgemm_f16 but the tensor core accumulates in
- * fp16 (tcgen05 D format f16, one rounding per k16 instruction) exactly like the reference's
+ * fp16 (wgmma D format f16, one rounding per k16 instruction) exactly like the reference's
  * HMMA.16816.F16 kernels (mma/basic/hgemm_mma.cu:67-73) and its cuBLAS CUBLAS_COMPUTE_16F op
  * (cublas/hgemm_cublas.cu:50-52).  Less accurate than the default fp32 accumulation; provided so
  * that outputs can be compared with the reference's bit for bit.  Select it for every mirror op
@@ -92,11 +88,11 @@ int b200_hgemm_f16_rows(const void* a_shard, const void* b, void* c_full, int ro
  * finished tile to the other GPUs while the remaining tiles are still being computed.  At least one
  * of the two target descriptions must be given (else B200_EINVAL):
  *   c_full_peers / n_peers (1..7) : peer-mapped C buffers of the other GPUs.  This is the default
- *                              transport: each finished 64x32 box is staged in shared memory and
- *                              TMA-stored to c_full and to every peer (NVLink P2P).
+ *                              transport: the epilogue stores every value to c_full and to every
+ *                              peer (NVLink P2P).
  *   c_full_multicast         : an NVLS multicast mapping of the symmetric C buffer.  Used when no
- *                              peers are given (one multimem.st per 16 bytes reaches every GPU, this
- *                              one included), or when B200_FUSED_EPILOGUE=direct|mc selects it.
+ *                              peers are given (one multimem.st reaches every GPU, this one
+ *                              included), or when B200_FUSED_EPILOGUE=direct|mc selects it.
  * n_peers > 0 with c_full_peers == NULL is rejected.  The caller closes the step with a cross-GPU
  * barrier and must not let a peer overwrite a C buffer that is still being read (leetcuda_b200/dist.py
  * alternates two symmetric buffers). */
@@ -119,15 +115,12 @@ int b200_hgemm_f16_rows_fused(const void* a_shard, const void* b, void* c_full, 
  * Constraints: D % 8 == 0 and D <= 1024; any N >= 1 (N % 8 == 0 for v_transposed).  For
  * v_transposed with D > 128 V is first restored to [B,H,N,D] in a stream-ordered scratch
  * allocation (cudaMallocAsync / cudaFreeAsync on `stream`).
- * Kernels: D <= 128 the single-CTA two-query-tile kernel (persistent scheduling for D <= 64; a CTA-pair
- * variant with cta_group::2 M = 256 exists behind B200_ATTN_CG2=1 and measured slower); D = 256, 384, 512
- * the CTA-pair kernel with one 128-row query tile per cluster (cta_group::2, M = 128); every other
- * D <= 1024 the column-slab kernel.
+ * Kernel (wgmma, TMA, mbarrier): each CTA owns a query tile and a column slab of O — one slab of 64 / 128
+ * columns for D <= 64 / D <= 128, 256-column slabs above (each slab recomputes S).
  * Numerics: S, the softmax statistics and O in fp32, P rounded to fp16 before P.V (as the reference); the
- * exponentials are ex2.approx (MUFU) except, for D <= 128, a fixed quarter to third of the score pairs, which a
- * degree-3 polynomial on the FMA pipe evaluates with max. relative error 7.6e-5 — below the fp16 rounding P
- * receives next (tests/test_softmax_math.py).  Measured max |error| 2-3e-3 on adversarial inputs, 2e-4
- * typical, against the reference's own tolerance allclose(1e-2, 1e-2).
+ * exponentials are ex2.approx (MUFU) except, for D <= 128, a fixed quarter of the keys, which a degree-3 polynomial on
+ * the FMA pipe evaluates with max. relative error 7.6e-5 — below the fp16 rounding P receives next
+ * (tests/test_softmax_math.py).  Tolerance against the reference: allclose(1e-2, 1e-2), its own criterion.
  */
 int b200_fmha_fwd_f16(const void* q, const void* k, const void* v, void* o, int B, int H, int N,
                       int D, int v_transposed, float scale, void* stream);
@@ -141,7 +134,7 @@ int b200_fmha_fwd_f16_lse(const void* q, const void* k, const void* v, void* o, 
                           int H, int N, int D, int v_transposed, float scale, void* stream);
 
 /* ------------------------------------------------------------------ SGEMM (TF32)
- * C[M,N] (fp32) = A[M,K] (fp32) x B on the tensor cores through tcgen05 kind::tf32 with fp32
+ * C[M,N] (fp32) = A[M,K] (fp32) x B on the tensor cores through wgmma .tf32 with fp32
  * accumulation — the sibling of the HGEMM path (SURVEY §8f-2).  Replaces
  *   sgemm_wmma_m16n16k8_mma4x2_warp2x4_stages{,_dsmem}(a,b,c,stages,swizzle,swizzle_stride)
  *   (kernels/sgemm/sgemm_wmma_tf32_stage.cu:573-742, bound in kernels/sgemm/sgemm.cu:762-764).
@@ -216,7 +209,8 @@ int b200_rms_norm(const void* x, void* y, float g, int rows, int K, int dtype, v
  * i.e. b200_fmha_fwd_f16 followed by b200_rms_norm over rows of length D, without the round trip of O
  * through HBM (the row already sits in the registers of one thread when the epilogue runs).  rms_g <= 0
  * disables the normalisation (then identical to b200_fmha_fwd_f16_lse with an optional lse).  lse may be
- * NULL.  Supported for D <= 256 and for the CTA-pair kernel's head dims (384, 512); B200_ENOTSUP otherwise. */
+ * NULL.  Supported for D <= 256 and for D = 384, 512 (there the two 256-column slabs of a query tile run as a
+ * cluster of two CTAs and add up the row statistics through distributed shared memory); B200_ENOTSUP otherwise. */
 int b200_fmha_fwd_f16_rmsnorm(const void* q, const void* k, const void* v, void* o, float* lse, int B,
                               int H, int N, int D, int v_transposed, float scale, float rms_g, void* stream);
 

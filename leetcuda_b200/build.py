@@ -1,10 +1,9 @@
-"""In-tree build of the sm_100a shared library behind the C ABI.
+"""In-tree build of the sm_90a shared library behind the C ABI.
 
     python -m leetcuda_b200.build [--force] [--verbose]
 
-nvcc cross-compiles for sm_100a without a GPU.  The product is
-leetcuda_b200/libleetcuda_b200.so (git-ignored; it travels to the GPU box with
-the gpurun snapshot).  Objects are rebuilt only when a source or header is newer.
+nvcc cross-compiles for sm_90a without a GPU.  The product is
+leetcuda_b200/libleetcuda_b200.so (git-ignored).  Objects are rebuilt only when a source or header is newer.
 """
 from __future__ import annotations
 
@@ -24,7 +23,7 @@ SOURCES = ["capi_common.cu", "hgemm_capi.cu", "attn_capi.cu", "merge_capi.cu", "
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
     "-Xptxas", "-v",

@@ -4,130 +4,42 @@
 #include <string.h>
 
 #include "capi_common.cuh"
-#include "attn_sm100.cuh"
-#include "attn_slab_sm100.cuh"
-#include "attn_pair_sm100.cuh"
-#include "attn_cg2_sm100.cuh"
+#include "attn_sm90.cuh"
 
 namespace b200 { namespace host {
 int workspace(void** out, size_t bytes);
 } }
-
-#ifndef B200_ATTN_SPEC_DEFAULT
-#define B200_ATTN_SPEC_DEFAULT 0
-#endif
-// Measured defaults (profiles/r02_session2b.log, r02_session2c.log; B4 H32 N4096, TFLOPS):
-//   D = 128: single-CTA one-shot 1258-1279 | persistent 1236-1254 | speculative softmax 1212 (removed) | CTA pair (M=256) 946
-//   D = 64 : single-CTA one-shot 600-730   | persistent 740-790
-// The CTA-pair variant removes the shared-memory operand limit of Q.K^T (tools/umma_rate.cu) but every hand-shake of
-// the softmax <-> MMA chain then crosses the cluster, and that chain — not a pipe — is what bounds the kernel.
-#ifndef B200_ATTN_CG2_DEFAULT
-#define B200_ATTN_CG2_DEFAULT 0
-#endif
-#ifndef B200_ATTN_PAIR_PERSIST_DEFAULT
-#define B200_ATTN_PAIR_PERSIST_DEFAULT 0
-#endif
-#ifndef B200_ATTN_PERSIST_DEFAULT
-#define B200_ATTN_PERSIST_DEFAULT 0
-#endif
 
 namespace {
 
 using namespace b200;
 using b200::host::fail;
 
-template <int DP, bool kVT, int kStep, bool kPersist>
-int launch_fmha(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
-                const CUtensorMap& to, const attn::Params& p, int BH, cudaStream_t stream) {
-  // (the kernel is b200::attn::attn_fwd_kernel — the host-side names keep the C ABI's "fmha")
-  using C_ = attn::Cfg<DP>;
-  auto kern = attn::attn_fwd_kernel<DP, kVT, kStep, kPersist>;
-  static bool attr_set[64] = {false};
+template <int kDS, int kBN, int kWG, bool kVT>
+int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const attn::Params& p, int qtiles,
+                int BH, int smem, cudaStream_t stream) {
+  auto kern = attn::attn_fwd_kernel<kDS, kBN, kWG, kVT>;
+  static int attr_smem[64] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      C_::SMEM_BYTES));
-    attr_set[dev] = true;
-  }
-  dim3 grid((p.N + 2 * attn::BR - 1) / (2 * attn::BR), BH, 1);
-  if (kPersist) {
-    const int sms = host::sm_count();
-    grid = dim3(static_cast<unsigned>(p.total_items < sms ? p.total_items : sms), 1, 1);
-  }
-  // debug: B200_FMHA_TRACE=<file> dumps the clock64 timeline of CTA (0,0) (synchronous!)
-  const char* trace_path = getenv("B200_FMHA_TRACE");
-  attn::Params pp = p;
-  pp.trace = nullptr;
-  if (trace_path && trace_path[0]) {
-    const size_t n = 3 * 16 * 8;
-    B200_CUDA_OK(cudaMalloc(&pp.trace, n * 8));
-    B200_CUDA_OK(cudaMemset(pp.trace, 0, n * 8));
-    kern<<<grid, attn::kThreads, C_::SMEM_BYTES, stream>>>(tq, tk, tv, to, pp);
-    B200_CUDA_OK(cudaStreamSynchronize(stream));
-    unsigned long long h[3 * 16 * 8];
-    B200_CUDA_OK(cudaMemcpy(h, pp.trace, n * 8, cudaMemcpyDeviceToHost));
-    cudaFree(pp.trace);
-    if (FILE* f = fopen(trace_path, "w")) {
-      for (int r = 0; r < 3; ++r)
-        for (int j = 0; j < 16; ++j) {
-          fprintf(f, "%d %d", r, j);
-          for (int e = 0; e < 8; ++e) fprintf(f, " %llu", h[(r * 16 + j) * 8 + e]);
-          fprintf(f, "\n");
-        }
-      fclose(f);
-    }
-    host::count_launch();
-    return 0;
-  }
-  kern<<<grid, attn::kThreads, C_::SMEM_BYTES, stream>>>(tq, tk, tv, to, pp);
-  B200_CUDA_OK(cudaGetLastError());
-  host::count_launch();
-  return 0;
-}
-
-// 64 < D <= 128 on CTA pairs (attn_cg2_sm100.cuh): cluster of two CTAs = 512 query rows, cta_group::2 MMAs with M = 256
-template <bool kVT>
-int launch_attn_cg2(const void* q, const void* k, const void* v, void* o, const attn2::Params& p, uint64_t BH, int N, int D,
-                    cudaStream_t stream) {
-  CUtensorMap tq, tk, tv, to;
-  uint64_t dims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(N), BH};
-  uint64_t str[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(N) * D * 2};
-  uint32_t qbox[3] = {64, 128, 1};
-  uint32_t kbox[3] = {64, 64, 1};
-  int rc;
-  if ((rc = host::get_tmap(&tq, q, 3, dims, str, qbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&to, o, 3, dims, str, qbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&tk, k, 3, dims, str, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if (kVT) {
-    uint64_t vd[3] = {static_cast<uint64_t>(N), static_cast<uint64_t>(D), BH};
-    uint64_t vs[2] = {static_cast<uint64_t>(N) * 2, static_cast<uint64_t>(N) * D * 2};
-    if ((rc = host::get_tmap(&tv, v, 3, vd, vs, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  } else {
-    if ((rc = host::get_tmap(&tv, v, 3, dims, str, qbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  }
-  auto kern = attn2::attn_cg2_fwd_kernel<kVT>;
-  static bool attr_set[64] = {false};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, attn2::SMEM_BYTES));
-    attr_set[dev] = true;
+  if (dev >= 0 && dev < 64 && attr_smem[dev] < smem) {
+    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr_smem[dev] = smem;
   }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(2u * static_cast<unsigned>((N + 4 * attn2::BR - 1) / (4 * attn2::BR)), static_cast<unsigned>(BH), 1);
-  cfg.blockDim = dim3(attn2::kThreads, 1, 1);
-  cfg.dynamicSmemBytes = attn2::SMEM_BYTES;
+  cfg.gridDim = dim3(static_cast<unsigned>(qtiles * p.slabs), static_cast<unsigned>(BH), 1);
+  cfg.blockDim = dim3(attn::threads<kWG>(), 1, 1);
+  cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
   cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeClusterDimension;
-  attrs[0].val.clusterDim.x = 2;
+  attrs[0].id = cudaLaunchAttributeClusterDimension;   // the slabs of one query tile (fused RMS norm)
+  attrs[0].val.clusterDim.x = (p.rms_g > 0.f) ? static_cast<unsigned>(p.slabs) : 1u;
   attrs[0].val.clusterDim.y = 1;
   attrs[0].val.clusterDim.z = 1;
   cfg.attrs = attrs;
   cfg.numAttrs = 1;
-  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tq, tk, tv, to, p));
+  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tq, tk, tv, p));
   host::count_launch();
   return 0;
 }
@@ -150,132 +62,63 @@ __global__ void transpose_dn_to_nd_kernel(const __half* __restrict__ in, __half*
   }
 }
 
-// head dims 128 < D <= 1024: column-slab kernel (attn_slab_sm100.cuh)
-// 256 <= D <= 512, D % 128 == 0: one 128-row query tile per CTA PAIR (attn_pair_sm100.cuh)
-int fmha_pair(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int H, int N, int D,
-              float scale, cudaStream_t stream) {
+// Kernel shape per head dim (attn_sm90.cuh):
+//   D <= 64        one 64-column slab, 128-key blocks, two consumer warpgroups (128 query rows)
+//   64 < D <= 128  one 128-column slab, 64-key blocks, two consumer warpgroups
+//   128 < D        256-column slabs (S recomputed per slab), 64-key blocks, one consumer warpgroup (64 query rows)
+// The S, P and O fragments of a consumer thread have to fit its registers: ptxas gives a 384-thread CTA
+// 168 per thread, a 256-thread CTA 255 (O of a 256-column slab alone takes 128).
+int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int H, int N,
+                  int D, bool vt, float scale, cudaStream_t stream) {
   const uint64_t BH = static_cast<uint64_t>(B) * H;
-  attn_pair::Params p;
+  const int ds = D <= 64 ? 64 : (D <= 128 ? 128 : 256);
+  const int bn = ds == 64 ? 128 : 64;
+  const int wgs = ds == 256 ? 1 : 2;
+  attn::Params p;
   p.N = N;
-  p.num_kv = (N + attn_pair::BC - 1) / attn_pair::BC;
-  p.nq = D / 64;
-  p.n_hi = D - 256;
+  p.D = D;
+  p.nq = (D + 63) / 64;
+  p.num_kv = (N + bn - 1) / bn;
+  p.slabs = (D + ds - 1) / ds;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.lse = lse;
   p.rms_g = rms_g;
+  p.o_ptr = static_cast<__half*>(o);
+  if (rms_g > 0.f && D > 256 && !(D <= 512 && D % 128 == 0))
+    return fail(B200_ENOTSUP, "fused rms_norm: D=%d (supported: D <= 256, 384, 512)", D);
+  // ring: every slot that fits next to Q, at most 16 (two key blocks of K and V chunks at D = 512)
+  const int kMaxSmem = 227 * 1024;
+  const int slot = attn::slot_bytes(bn, ds, vt);
+  const int fixed = attn::smem_bytes(wgs, slot, p.nq, 0);
+  p.ring = (kMaxSmem - fixed) / (slot + 16);
+  if (p.ring > 16) p.ring = 16;
+  if (p.ring < 2) return fail(B200_ENOTSUP, "headdim not support! (D=%d)", D);
+  const int smem = attn::smem_bytes(wgs, slot, p.nq, p.ring);
+  const int qtiles = (N + 64 * wgs - 1) / (64 * wgs);
 
-  CUtensorMap tq, tk, tv, to;
+  CUtensorMap tq, tk, tv;
   uint64_t dims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(N), BH};
   uint64_t str[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(N) * D * 2};
   uint32_t qbox[3] = {64, 64, 1};
-  uint32_t kbox[3] = {64, 128, 1};
-  uint32_t vbox[3] = {64, 64, 1};
+  uint32_t kbox[3] = {64, static_cast<uint32_t>(bn), 1};
   int rc;
   if ((rc = host::get_tmap(&tq, q, 3, dims, str, qbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&to, o, 3, dims, str, qbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   if ((rc = host::get_tmap(&tk, k, 3, dims, str, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&tv, v, 3, dims, str, vbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-
-  // B200_ATTN_PAIR_PERSIST=0|1: one cluster per query tile / one cluster per SM pair walking the work items
-  static int persist = -1;
-  if (persist < 0) {
-    const char* e = getenv("B200_ATTN_PAIR_PERSIST");
-    persist = (e && e[0] == '0') ? 0 : ((e && e[0] == '1') ? 1 : B200_ATTN_PAIR_PERSIST_DEFAULT);
+  if (vt) {
+    uint64_t vd[3] = {static_cast<uint64_t>(N), static_cast<uint64_t>(D), BH};
+    uint64_t vs[2] = {static_cast<uint64_t>(N) * 2, static_cast<uint64_t>(N) * D * 2};
+    uint32_t vb[3] = {64, static_cast<uint32_t>(ds), 1};
+    if ((rc = host::get_tmap(&tv, v, 3, vd, vs, vb, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  } else {
+    if ((rc = host::get_tmap(&tv, v, 3, dims, str, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   }
-  p.o_ptr = static_cast<__half*>(o);
-  p.qtiles = (N + attn_pair::BR - 1) / attn_pair::BR;
-  p.total_items = p.qtiles * static_cast<int>(BH);
-  const int smem = attn_pair::smem_bytes(p.nq);
-  auto kern = persist ? attn_pair::attn_pair_fwd_kernel<true> : attn_pair::attn_pair_fwd_kernel<false>;
-  static int attr_smem[64][2] = {{0}};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && attr_smem[dev][persist] < smem) {
-    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_smem[dev][persist] = smem;
-  }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(2u * static_cast<unsigned>(p.qtiles), static_cast<unsigned>(BH), 1);
-  if (persist) {
-    const int slots = host::sm_count() / 2;
-    cfg.gridDim = dim3(2u * static_cast<unsigned>(p.total_items < slots ? p.total_items : slots), 1, 1);
-  }
-  cfg.blockDim = dim3(attn_pair::kThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeClusterDimension;
-  attrs[0].val.clusterDim.x = 2;
-  attrs[0].val.clusterDim.y = 1;
-  attrs[0].val.clusterDim.z = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = 1;
-  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tq, tk, tv, to, p));
-  host::count_launch();
-  return 0;
-}
-
-// B200_ATTN_LARGE_D=slab keeps the column-slab kernel for every D > 128 (A/B runs, bring-up)
-bool pair_kernel_enabled() {
-  static int cached = -1;
-  if (cached < 0) {
-    const char* e = getenv("B200_ATTN_LARGE_D");
-    cached = (e && strcmp(e, "slab") == 0) ? 0 : 1;
-  }
-  return cached == 1;
-}
-
-int fmha_large_d(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int H, int N, int D,
-                 float scale, cudaStream_t stream) {
-  // D = 256 also runs on the pair kernel (B200_ATTN_LARGE_D=pair256) but measured slower there than on one slab per CTA
-  // (790 / 974 vs 912 / 1163 TFLOPS at N = 2048 / 4096, profiles/r02_session2d.log): with half the MMA work per key the
-  // softmax of a 256-key tile is the longer leg
-  static int pair256 = -1;
-  if (pair256 < 0) { const char* e = getenv("B200_ATTN_LARGE_D"); pair256 = (e && strcmp(e, "pair256") == 0) ? 1 : 0; }
-  if (D >= (pair256 ? 256 : 257) && D <= 512 && D % 128 == 0 && pair_kernel_enabled())
-    return fmha_pair(q, k, v, o, lse, rms_g, B, H, N, D, scale, stream);
-  const uint64_t BH = static_cast<uint64_t>(B) * H;
-  attn_slab::Params p;
-  p.N = N;
-  p.num_kv = (N + attn_slab::BC - 1) / attn_slab::BC;
-  p.nq = (D + 63) / 64;
-  p.dsplit = (D + 255) / 256;
-  p.dv = (((D + p.dsplit - 1) / p.dsplit) + 63) / 64 * 64;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  p.lse = lse;
-  p.rms_g = rms_g;
-  p.D = D;
-  if (rms_g > 0.f && p.dsplit > 1)
-    return fail(B200_ENOTSUP, "fused rms_norm needs the whole output row in one CTA: D=%d is served by %d column slabs", D, p.dsplit);
-  if (p.nq > attn_slab::kMaxDChunks) return fail(B200_ENOTSUP, "headdim not support! (D=%d > 1024)", D);
-
-  CUtensorMap tq, tk, tv, to;
-  uint64_t dims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(N), BH};
-  uint64_t str[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(N) * D * 2};
-  const bool wide = p.nq <= attn_slab::kMaxQChunks;      // Q resident: 32 KiB ring slots, V boxes of 64 keys
-  uint32_t box[3] = {64, 128, 1};
-  uint32_t vbox[3] = {64, static_cast<uint32_t>(wide ? 64 : 32), 1};
-  int rc;
-  if ((rc = host::get_tmap(&tq, q, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&tk, k, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&to, o, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&tv, v, 3, dims, str, vbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-
-  const int smem = attn_slab::smem_bytes(p.nq);
-  auto kern = wide ? attn_slab::attn_slab_fwd_kernel<true> : attn_slab::attn_slab_fwd_kernel<false>;
-  static int attr_smem[64][2] = {{0}};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && attr_smem[dev][wide] < smem) {
-    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_smem[dev][wide] = smem;
-  }
-  dim3 grid(((N + attn_slab::BR - 1) / attn_slab::BR) * p.dsplit, static_cast<unsigned>(BH), 1);
-  kern<<<grid, attn_slab::kThreads, smem, stream>>>(tq, tk, tv, to, p);
-  B200_CUDA_OK(cudaGetLastError());
-  host::count_launch();
-  return 0;
+  const int bh = static_cast<int>(BH);
+  if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, stream)
+                          : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, stream);
+  if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, stream)
+                           : launch_attn<128, 64, 2, false>(tq, tk, tv, p, qtiles, bh, smem, stream);
+  if (vt) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with D=%d)", D);
+  return launch_attn<256, 64, 1, false>(tq, tk, tv, p, qtiles, bh, smem, stream);
 }
 
 int fmha_impl(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int N, int D,
@@ -307,88 +150,13 @@ int fmha_impl(const void* q, const void* k, const void* v, void* o, float* lse, 
       if (le != cudaSuccess) rc = fail(B200_ECUDA, "transpose launch failed: %s", cudaGetErrorString(le));
       else {
         host::count_launch();
-        rc = fmha_large_d(q, k, ws, o, lse, rms_g, B, H, N, D, scale, stream);
+        rc = fmha_dispatch(q, k, ws, o, lse, rms_g, B, H, N, D, false, scale, stream);
       }
       cudaFreeAsync(ws, stream);
       return rc;
     }
-    return fmha_large_d(q, k, v, o, lse, rms_g, B, H, N, D, scale, stream);
   }
-  const int DP = D <= 64 ? 64 : 128;
-  const uint64_t BH = static_cast<uint64_t>(B) * H;
-  {
-    // CTA-pair kernel for 64 < D <= 128 whenever a pair's 512 query rows are (mostly) real rows;
-    // B200_ATTN_CG2=0|1 overrides (A/B runs)
-    static int cg2 = -1;
-    if (cg2 < 0) {
-      const char* e = getenv("B200_ATTN_CG2");
-      cg2 = (e && e[0] == '0') ? 0 : ((e && e[0] == '1') ? 1 : B200_ATTN_CG2_DEFAULT);
-    }
-    if (cg2 && DP == 128 && (N % 512 == 0 || N >= 2048)) {
-      attn2::Params p2;
-      p2.N = N;
-      p2.D = D;
-      p2.num_kv = (N + attn2::BC - 1) / attn2::BC;
-      p2.scale_log2 = scale * 1.4426950408889634f;
-      p2.lse = lse;
-      p2.rms_g = rms_g;
-      return v_transposed ? launch_attn_cg2<true>(q, k, v, o, p2, BH, N, D, stream)
-                          : launch_attn_cg2<false>(q, k, v, o, p2, BH, N, D, stream);
-    }
-  }
-
-  attn::Params p;
-  p.N = N;
-  p.D = D;
-  p.num_kv = (N + attn::BC - 1) / attn::BC;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  p.lse = lse;
-  p.rms_g = rms_g;
-
-  CUtensorMap tq, tk, tv, to;
-  uint64_t dims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(N), BH};
-  uint64_t str[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(N) * D * 2};
-  uint32_t box[3] = {64, 128, 1};
-  int rc;
-  if ((rc = host::get_tmap(&tq, q, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&tk, k, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&to, o, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if (v_transposed) {
-    uint64_t vd[3] = {static_cast<uint64_t>(N), static_cast<uint64_t>(D), BH};
-    uint64_t vs[2] = {static_cast<uint64_t>(N) * 2, static_cast<uint64_t>(N) * D * 2};
-    uint32_t vb[3] = {64, static_cast<uint32_t>(DP), 1};
-    if ((rc = host::get_tmap(&tv, v, 3, vd, vs, vb, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  } else {
-    if ((rc = host::get_tmap(&tv, v, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  }
-  const int bh = static_cast<int>(BH);
-  // B200_ATTN_SPEC=0|2 picks the softmax step (attn_sm100.cuh, kStep: 0 classic, 2 sum-checked speculative);
-  // B200_ATTN_PERSIST=0|1: one CTA per work item / one CTA per SM walking the work items
-  static int spec = -1, persist = -1;
-  if (spec < 0) {
-    const char* e = getenv("B200_ATTN_SPEC");
-    spec = (e && e[0] == '2') ? 2 : ((e && e[0] == '0') ? 0 : B200_ATTN_SPEC_DEFAULT);
-    const char* f = getenv("B200_ATTN_PERSIST");
-    persist = (f && f[0] == '0') ? 0 : ((f && f[0] == '1') ? 1 : -1);   // -1: per head dim (below)
-  }
-  const int use_persist = persist >= 0 ? persist : (DP == 64 ? 1 : B200_ATTN_PERSIST_DEFAULT);
-  p.o_ptr = static_cast<__half*>(o);
-  p.qpairs = (N + 2 * attn::BR - 1) / (2 * attn::BR);
-  p.total_items = p.qpairs * bh;
-  switch ((DP == 64 ? 0 : 8) + (v_transposed ? 4 : 0) + spec + (use_persist ? 1 : 0)) {   // spec is 0 or 2
-#define B200_ATTN_CASE(n, dp, vt, sp, pe) \
-    case n: return launch_fmha<dp, vt, sp, pe>(tq, tk, tv, to, p, bh, stream);
-#define B200_ATTN_CASES(n0, dp, vt)                                                             \
-    B200_ATTN_CASE(n0 + 0, dp, vt, 0, false) B200_ATTN_CASE(n0 + 1, dp, vt, 0, true)            \
-    B200_ATTN_CASE(n0 + 2, dp, vt, 2, false) B200_ATTN_CASE(n0 + 3, dp, vt, 2, true)
-    B200_ATTN_CASES(0, 64, false)
-    B200_ATTN_CASES(4, 64, true)
-    B200_ATTN_CASES(8, 128, false)
-    B200_ATTN_CASES(12, 128, true)
-#undef B200_ATTN_CASES
-#undef B200_ATTN_CASE
-  }
-  return fail(B200_EINVAL, "fmha: internal dispatch error");
+  return fmha_dispatch(q, k, v, o, lse, rms_g, B, H, N, D, v_transposed != 0, scale, stream);
 }
 
 }  // namespace

@@ -235,7 +235,7 @@ int b200_rope_f32(const float* x, float* out, int seq_len, int hidden, void* str
   const unsigned lanes = (groups <= 256u && 256u % groups == 0u) ? groups : 256u;
   const unsigned rows_per_step = 256u / lanes;
   // one-shot grid (one row step per CTA; the loop in the kernel only wraps beyond 2^31 CTAs): for streaming kernels the
-  // block scheduler beat a persistent grid-stride loop by 10 % on this chip (merge_capi.cu, profiles/r02_session2e.log)
+  // block scheduler beat a persistent grid-stride loop (measured on the B200 this was first written for; not re-measured)
   size_t blocks = (static_cast<size_t>(seq_len) + rows_per_step - 1) / rows_per_step;
   const size_t cap = 0x7FFFFFFFull;
   if (blocks > cap) blocks = cap;
@@ -263,7 +263,7 @@ int b200_rope_qk_f16(const void* q, const void* k, void* q_out, void* k_out, int
   size_t blocks = (rows + rows_per_step - 1) / rows_per_step;
   // persistent grid here (x 2 tensors in grid.y = 8 CTAs per SM): with four pairs per pack this kernel is bound by
   // the sincosf / exp2f work, and a thread that keeps its column group amortises the frequencies over many rows
-  // (one-shot grid: 3.04 TB/s, persistent: 4.61 TB/s; profiles/r02_session2d.log, r02_session2f.log)
+  // (measured on the B200 this was first written for; not re-measured on H100)
   const size_t cap = static_cast<size_t>(b200::host::sm_count()) * 4;
   if (blocks > cap) blocks = cap;
   rope_qk_f16_kernel<<<dim3(static_cast<unsigned>(blocks), 2, 1), 256, 0, stream>>>(

@@ -12,12 +12,8 @@
 // Layout: one thread per 16-byte pack of the output, ONE-SHOT grid (packs / 256 CTAs of 256 threads, 32-bit index
 // arithmetic whenever the pack count fits): both 128-bit L1-bypassing loads of a pack are issued before the two
 // lse values are fetched.  Every thread of a row evaluates the row's two weights itself (a warp executes those few
-// instructions once for all its lanes either way).  Measured on one box, order-rotated against the reference's
-// kernel rebuilt for sm_100a (0.2846 ms = 5.75 TB/s at T 131072, H 16, D 128, fp16; profiles/r02_session2e.log):
-//     one-shot grid + streaming accesses   0.2811 ms  5.82 TB/s   <- default
-//     one-shot grid + plain accesses       0.2829 ms  5.78 TB/s
-//     persistent grid (148 x 8 CTAs, grid-stride) + streaming accesses   0.3156 ms  5.19 TB/s  (round 1's default)
-//     a row-per-lane-group layout (weights computed by one lane per row, broadcast by shuffle)   0.324 ms
+// instructions once for all its lanes either way).  On the B200 this was first written for, that layout beat a
+// persistent grid-stride loop, plain (cached) accesses and a row-per-lane-group layout; not re-measured on H100.
 // i.e. for this two-reads-one-write stream the hardware's block scheduler spreads the three address streams
 // better than a lock-step grid-stride loop, and the kernel lives off independent threads, not instruction count.
 //

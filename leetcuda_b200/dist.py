@@ -94,7 +94,7 @@ class RowShardedHgemm:
         return self.c_full
 
     def fused(self, a_shard: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-        """GEMM whose epilogue delivers each finished tile to every GPU (TMA stores to the peer
+        """GEMM whose epilogue delivers each finished tile to every GPU (stores to the peer
         mappings, or through the NVLS multicast mapping), closed by a symmetric-memory barrier:
         after it, the returned [world*rows, N] tensor holds the complete C on every rank.
 

@@ -1,8 +1,8 @@
 """Drop-in mirror of ffpa-attn's python package (`ffpa_attn`) and extension (`pyffpa_cuda`).
 
-reference: /root/reference/ffpa-attn/ffpa_attn/interface.py:1-68,
-           /root/reference/ffpa-attn/ffpa_attn/__init__.py,
-           /root/reference/ffpa-attn/csrc/pybind/ffpa_attn_api.cc:8-16
+reference: ffpa-attn/ffpa_attn/interface.py:1-68,
+           ffpa-attn/ffpa_attn/__init__.py,
+           ffpa-attn/csrc/pybind/ffpa_attn_api.cc:8-16
 
 ``ffpa(q, k, v, o=None, num_stages=2, level=L1, acc=FP32) -> o`` and the two raw ops
 ``ffpa_mma_acc_{f16,f32}_L1(Q, K, V, O, stages)``; Q,K,V,O fp16 ``[B,H,N,D]``.

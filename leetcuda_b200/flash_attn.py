@@ -1,6 +1,6 @@
 """Drop-in mirror of the reference's FlashAttention extension module (`flash_attn_lib`).
 
-Every name bound in /root/reference/kernels/flash-attn/pybind/flash_attn.cc:168-224
+Every name bound in the reference's kernels/flash-attn/pybind/flash_attn.cc:168-224
 exists here with the same signature and error behaviour:
 
 * 28 ops  ``op(Q, K, V, O, stages) -> None``  (6 basic, 4 acc_f32, 15 swizzle, 3 "others")
@@ -11,11 +11,11 @@ Q, K, O are fp16 contiguous ``[B,H,N,D]``; V is ``[B,H,N,D]`` except for the thr
 pre-transposed ``[B,H,D,N]`` (flash_attn_mma.py:441-442,716,807,898).  O is written
 in place.  Non-causal, scale = 1/sqrt(D) (flash_attn_mma_split_q.cu:79).
 
-All of them run the same fused sm_100a kernel through ``b200_fmha_fwd_f16``;
+All of them run the same fused sm_90a kernel through ``b200_fmha_fwd_f16``;
 ``stages`` is a hint of the reference's cp.async pipeline and is ignored.  The
 reference's family differences (which of Q/K/V share smem, fp16 vs fp32 MMA
 accumulators) are implementation details of its mma.sync kernels: here S and O
-always accumulate in fp32 in TMEM, which is at least as accurate as every variant.
+always accumulate in fp32 in registers, which is at least as accurate as every variant.
 """
 from __future__ import annotations
 
@@ -140,7 +140,7 @@ def _make(name: str):
         fmha_fwd(Q, K, V, O, v_transposed=vt)
     op.__name__ = op.__qualname__ = name
     op.__doc__ = (f"{name}(Q, K, V, O, stages) -> None  "
-                  f"[V is {'[B,H,D,N]' if vt else '[B,H,N,D]'}; stages ignored; sm_100a fused kernel]")
+                  f"[V is {'[B,H,D,N]' if vt else '[B,H,N,D]'}; stages ignored; sm_90a fused kernel]")
     return op
 
 

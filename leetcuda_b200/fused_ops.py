@@ -70,9 +70,10 @@ def attn_rope(Q, K, V, O, *, rms_g: float = 0.0, lse=None) -> None:
         fmha_fwd(q_r, k_r, V, O, lse=lse)
 
 
-def bench_rows(torch_mod, dev, steps, peak_hbm, peak_src, cuda_time_ms):
+def bench_rows(torch_mod, dev, steps, peak_hbm, peak_src, cuda_time_ms, dump=lambda name, t: None):
     """bench.py rows of §8f-4: rope and rms_norm against the HBM roofline, and the fused attention epilogue
-    against attention + a separate rms_norm pass."""
+    against attention + a separate rms_norm pass.  dump(name, tensor) receives what the last timed step of each
+    row computed."""
     from . import flash_attn, rms_norm as RN, rope as RP
     t = torch_mod
     sync = lambda: t.cuda.synchronize()
@@ -84,6 +85,7 @@ def bench_rows(torch_mod, dev, steps, peak_hbm, peak_src, cuda_time_ms):
     for i in range(3):
         RP.rope_f32x4_pack(xs[i % 2], ys[i % 2])
     ms = cuda_time_ms(lambda i: RP.rope_f32x4_pack(xs[i % 2], ys[i % 2]), steps, sync) / steps
+    dump("rope_out", ys[(steps - 1) % 2])
     nbytes = 2 * S * Hd * 4
     rows.append({"metric": "rope GB/s @seq65536 hidden2048 fp32 (read + write)", "value": nbytes / ms / 1e6, "unit": "GB/s",
                  "ms_per_step": ms, "config": {"workload": "rope_seq65536_hidden2048_fp32", "op": "rope_f32x4_pack"},
@@ -98,6 +100,7 @@ def bench_rows(torch_mod, dev, steps, peak_hbm, peak_src, cuda_time_ms):
     for i in range(3):
         RN.rms_norm_f16x8_pack_f32(xs[i % 2], ys[i % 2], 1.0)
     ms = cuda_time_ms(lambda i: RN.rms_norm_f16x8_pack_f32(xs[i % 2], ys[i % 2], 1.0), steps, sync) / steps
+    dump("rms_norm_out", ys[(steps - 1) % 2])
     nbytes = 2 * R * Kk * 2
     rows.append({"metric": "rms_norm GB/s @rows131072 K2048 fp16 (read + write)", "value": nbytes / ms / 1e6, "unit": "GB/s",
                  "ms_per_step": ms, "config": {"workload": "rms_norm_rows131072_K2048_fp16", "op": "rms_norm_f16x8_pack_f32"},
@@ -112,6 +115,8 @@ def bench_rows(torch_mod, dev, steps, peak_hbm, peak_src, cuda_time_ms):
     for i in range(3):
         rope_qk(sets[i % 2][0], sets[i % 2][1], qr, kr)
     ms = cuda_time_ms(lambda i: rope_qk(sets[i % 2][0], sets[i % 2][1], qr, kr), steps, sync) / steps
+    dump("rope_qk_q", qr)
+    dump("rope_qk_k", kr)
     nbytes = 4 * B * H * N * D * 2
     rows.append({"metric": "rope of q,k GB/s @B4H32N4096D128 fp16 (read + write)", "value": nbytes / ms / 1e6, "unit": "GB/s",
                  "ms_per_step": ms, "config": {"workload": "rope_qk_B4_H32_N4096_D128_fp16", "op": "rope_qk"},
@@ -125,6 +130,7 @@ def bench_rows(torch_mod, dev, steps, peak_hbm, peak_src, cuda_time_ms):
     for i in range(3):
         attn_rmsnorm(*sets[i % 2], o, 1.0)
     f_ms = cuda_time_ms(lambda i: attn_rmsnorm(*sets[i % 2], o, 1.0), steps, sync) / steps
+    dump("attn_rmsnorm_o", o)
 
     def unfused(i):
         flash_attn.fmha_fwd(*sets[i % 2], o)
@@ -132,6 +138,7 @@ def bench_rows(torch_mod, dev, steps, peak_hbm, peak_src, cuda_time_ms):
     for i in range(3):
         unfused(i)
     u_ms = cuda_time_ms(unfused, steps, sync) / steps
+    dump("attn_then_rms_norm_o", o2)
     fl = 4.0 * B * H * N * N * D
     rows.append({"metric": "attention + fused RMS-norm epilogue TFLOPS @B4H32N4096D128", "value": fl / f_ms / 1e9, "unit": "TFLOPS",
                  "ms_per_step": f_ms, "config": {"workload": "attn_rmsnorm_B4_H32_N4096_D128_fp16", "op": "attn_rmsnorm"},

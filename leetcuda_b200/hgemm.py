@@ -1,6 +1,6 @@
 """Drop-in mirror of the reference's HGEMM extension module (`toy_hgemm` / `hgemm_lib`).
 
-Every name bound in /root/reference/kernels/hgemm/pybind/hgemm.cc:124-182 exists
+Every name bound in the reference's kernels/hgemm/pybind/hgemm.cc:124-182 exists
 here with the same signature, argument meaning and error behaviour:
 
 * 25 three-argument ops            ``op(a, b, c) -> None``
@@ -12,11 +12,11 @@ place.  For the NN ops ``b`` is ``[K,N]`` row-major; for the ``*_tn*`` ops ``b``
 still has torch shape ``[K,N]`` but its storage is ``[N,K]`` row-major, exactly what
 the reference's ``as_col_major`` produces (kernels/hgemm/tools/utils.py:151-156).
 
-All of them run the same sm_100a tcgen05/TMA kernel through the C ABI
+All of them run the same sm_90a wgmma/TMA kernel through the C ABI
 (``b200_hgemm_f16``); ``stages``/``swizzle``/``swizzle_stride`` are tuning hints of
 the reference's own tiling (hgemm.py:198-208) and are accepted and ignored.
 Unlike the reference (fp16 accumulation, e.g. mma/basic/hgemm_mma.cu:67-73) the
-accumulation is fp32 in TMEM; see DESIGN.md "Numerics".
+accumulation is fp32 in the wgmma accumulator registers; see DESIGN.md "Numerics".
 """
 from __future__ import annotations
 
@@ -89,7 +89,7 @@ def hgemm(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, *, tn: bool = False
 
     ``tn=False``: ``b`` is ``[K,N]`` row-major.  ``tn=True``: ``b`` has shape ``[K,N]``
     but holds ``[N,K]`` row-major storage (the reference's TN convention).
-    ``acc``: ``"f32"`` (default, TMEM fp32 accumulators) or ``"f16"`` (the reference's fp16
+    ``acc``: ``"f32"`` (default, fp32 accumulators) or ``"f16"`` (the reference's fp16
     accumulation, for bit-level comparison with its kernels).
     """
     _check_half(a)
@@ -154,7 +154,7 @@ def _make_3arg(name: str, tn: bool):
     def op(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor) -> None:
         hgemm(a, b, c, tn=tn)
     op.__name__ = op.__qualname__ = name
-    op.__doc__ = f"{name}(a, b, c) -> None  [{'TN' if tn else 'NN'}; sm_100a tcgen05 kernel]"
+    op.__doc__ = f"{name}(a, b, c) -> None  [{'TN' if tn else 'NN'}; sm_90a wgmma kernel]"
     return op
 
 
@@ -164,7 +164,7 @@ def _make_staged(name: str, tn: bool):
         hgemm(a, b, c, tn=tn)
     op.__name__ = op.__qualname__ = name
     op.__doc__ = (f"{name}(a, b, c, stages, swizzle, swizzle_stride) -> None  "
-                  f"[{'TN' if tn else 'NN'}; hints ignored; sm_100a tcgen05 kernel]")
+                  f"[{'TN' if tn else 'NN'}; hints ignored; sm_90a wgmma kernel]")
     return op
 
 

@@ -5,7 +5,7 @@ Reference: kernels/openai-triton/merge-attn-states/cuda_merge_attn_states.cu:158
 and cuda_merge_attn_states.py:24-35 wraps it as
 ``merge_attn_states_cuda(output, prefix_output, prefix_lse, suffix_output, suffix_lse, output_lse=None)``.
 Both spellings exist here (``lib.merge_attn_states_cuda`` is the raw binding order) and run the
-sm_100a kernel through the C ABI (``b200_merge_attn_states``).
+sm_90a kernel through the C ABI (``b200_merge_attn_states``).
 
 ``output`` / ``prefix_output`` / ``suffix_output``: ``[num_tokens, num_heads, head_size]`` fp32, fp16
 or bf16; the lse tensors ``[num_heads, num_tokens]`` fp32.  ``output`` (and ``output_lse``) are written

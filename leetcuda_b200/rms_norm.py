@@ -4,7 +4,7 @@ Nine ops ``op(x, y, g)`` (kernels/rms-norm/rms_norm.cu:493-771, bound :781-789):
 fp32 (``rms_norm_f32``, ``rms_norm_f32x4``) or fp16 (the seven ``rms_norm_f16*`` names), scalar gain
 ``g``; ``y = x * rsqrt(mean(x^2, dim=1) + 1e-5) * g``, written in place.  The names encode the
 reference's vector width and whether its statistics are fp16 or fp32; here every name runs the same
-HBM-bound sm_100a kernel (``b200_rms_norm``) with fp32 statistics, which is at least as accurate as each
+HBM-bound sm_90a kernel (``b200_rms_norm``) with fp32 statistics, which is at least as accurate as each
 variant.
 """
 from __future__ import annotations
@@ -42,7 +42,7 @@ def _make(name: str, dtype):
             raise RuntimeError("values must be torch::kFloat32" if dtype == torch.float32 else "values must be torch::kHalf")
         rms_norm(x, y, g)
     op.__name__ = op.__qualname__ = name
-    op.__doc__ = f"{name}(x, y, g) -> None  [sm_100a kernel, fp32 statistics]"
+    op.__doc__ = f"{name}(x, y, g) -> None  [sm_90a kernel, fp32 statistics]"
     return op
 
 

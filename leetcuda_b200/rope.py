@@ -2,7 +2,7 @@
 
 ``rope_f32(x, out)``, ``rope_f32_v2(x, out)``, ``rope_f32x4_pack(x, out)`` (kernels/rope/rope.cu:88-125):
 ``x``, ``out`` fp32 ``[seq_len, hidden]``; the three names differ only in the reference's thread indexing,
-here they run the same HBM-bound sm_100a kernel through ``b200_rope_f32``.  ``out`` is written in place.
+here they run the same HBM-bound sm_90a kernel through ``b200_rope_f32``.  ``out`` is written in place.
 """
 from __future__ import annotations
 

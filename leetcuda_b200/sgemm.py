@@ -1,12 +1,12 @@
 """Drop-in mirror of the reference's SGEMM extension module (`sgemm_lib`), SURVEY §8f-2.
 
-Every name bound in /root/reference/kernels/sgemm/sgemm.cu:743-765 exists here with the same
+Every name bound in the reference's kernels/sgemm/sgemm.cu:743-765 exists here with the same
 signature, argument meaning and error behaviour.  ``a`` is ``[M,K]``, ``b`` is ``[K,N]``, ``c`` is
 ``[M,N]``, all fp32 row-major; ``c`` is written in place.
 
 * the two TF32 tensor-core ops
   ``sgemm_wmma_m16n16k8_mma4x2_warp2x4_stages{,_dsmem}(a, b, c, stages, swizzle, swizzle_stride)``
-  (sgemm_wmma_tf32_stage.cu:573-742) run the sm_100a tcgen05 ``kind::tf32`` kernel through the
+  (sgemm_wmma_tf32_stage.cu:573-742) run the sm_90a wgmma ``.tf32`` kernel through the
   C ABI (``b200_sgemm_tf32``).  Like the reference they first round ``a`` and ``b`` to TF32 **in
   place** (sgemm_wmma_tf32_stage.cu:44-60, 586-592); the hints are accepted and ignored.
 * ``sgemm_cublas`` / ``sgemm_cublas_tf32`` (sgemm_cublas.cu:17-43) stay vendor calls: they are the
@@ -14,7 +14,7 @@ signature, argument meaning and error behaviour.  ``a`` is ``[M,K]``, ``b`` is `
 * the 13 CUDA-core fp32 ops (sgemm.cu:743-760, sgemm_async.cu) compute a full-precision fp32 product (FFMA
   accumulation, ~2e-6 relative at K = 1024).  No tensor-core path reproduces that: a TF32 product is at 1e-3,
   and the 3xTF32 split offered here as ``sgemm_3xtf32`` (``b200_sgemm_3xtf32``: each operand = two exact TF32
-  numbers, three partial products in ONE tcgen05 ``kind::tf32`` GEMM over K' = 3K) removes the operand rounding
+  numbers, three partial products in ONE wgmma ``.tf32`` GEMM over K' = 3K) removes the operand rounding
   but keeps the tensor core's truncating accumulation — measured 5e-5 relative at K = 1024..4096
   (tests/test_sgemm_gpu.py), 20x better than TF32 and 20x worse than FFMA.  So by default these 13 names are
   VENDOR ROWS (cuBLAS fp32 through torch.matmul, said so in every docstring) and keep the reference's
@@ -123,7 +123,7 @@ def _make_tf32_staged(name: str):
         sgemm_tf32(a, b, c, round_inputs=True)
     op.__name__ = op.__qualname__ = name
     op.__doc__ = (f"{name}(a, b, c, stages, swizzle, swizzle_stride) -> None  "
-                  "[TF32 tensor cores, inputs rounded in place; hints ignored; sm_100a tcgen05 kernel]")
+                  "[TF32 tensor cores, inputs rounded in place; hints ignored; sm_90a wgmma kernel]")
     return op
 
 

@@ -1,9 +1,8 @@
-"""TEST INFRASTRUCTURE — build the UNMODIFIED reference kernels for sm_100a.
+"""TEST INFRASTRUCTURE — build the UNMODIFIED reference kernels for sm_90a.
 
-Compiles the reference's own CUDA sources *where they lie* under /root/reference
-(nothing is copied) together with the small binding files in this directory into
-python extension modules under oracle/_ref/ (git-ignored, but shipped to the GPU
-box with the gpurun snapshot):
+Compiles the reference's own CUDA sources *where they lie* in the reference checkout (/root/reference,
+or $LEETCUDA_REFERENCE; nothing is copied) together with the small binding files in this
+directory into python extension modules under oracle/_ref/ (git-ignored):
 
     oracle/_ref/ref_hgemm/ref_hgemm.so    kernels/hgemm       (all tensor-core ops + cuBLAS op)
     oracle/_ref/ref_fa/ref_fa.so          kernels/flash-attn  (split-q, share-qkv{,acc_f32,swizzle_qkv}, tiling-qkv)
@@ -15,13 +14,13 @@ box with the gpurun snapshot):
 
 Flags follow the reference's JIT builds (kernels/hgemm/tools/utils.py:62-98,
 kernels/flash-attn/flash_attn_mma.py:151-195, ffpa-attn/env.py:312-343, kernels/sgemm/sgemm.py:11-31) with the arch
-set to sm_100a.  The modules are the on-box comparator and the source of the
+set to sm_90a.  The modules are the on-box comparator and the source of the
 golden vectors under tests/golden/ (oracle/gen_golden.py); the product never
 loads them.
 
 `scripts` stages the reference's own BENCH / TEST SCRIPTS (python files only, byte for byte) under
-oracle/_ref/scripts/ in their original directory layout, so that the GPU box — which has no
-/root/reference — can run them unmodified against the mirror (tools/run_reference_script.py,
+oracle/_ref/scripts/ in their original directory layout, so that a GPU machine without a reference
+checkout can run them unmodified against the mirror (tools/run_reference_script.py,
 tests/test_reference_scripts_gpu.py).  Like everything under oracle/_ref/ they are never committed.
 
     python oracle/build_ref.py [hgemm] [fa] [ffpa] [sgemm] [merge] [rope] [rmsnorm] [scripts]
@@ -34,7 +33,15 @@ from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
 OUT = HERE / "_ref"
+# the reference checkout (xlite-dev/LeetCUDA) the comparators are built from; $LEETCUDA_REFERENCE overrides the default
 REF = Path(os.environ.get("LEETCUDA_REFERENCE", "/root/reference"))
+
+
+def reference_present() -> bool:
+    try:
+        return REF.is_dir()
+    except OSError:   # e.g. a path under a directory this user may not enter
+        return False
 
 COMMON = [
     "-O3", "-std=c++17",
@@ -42,12 +49,12 @@ COMMON = [
     "-U__CUDA_NO_HALF2_OPERATORS__", "-U__CUDA_NO_BFLOAT16_CONVERSIONS__",
     "--expt-relaxed-constexpr", "--expt-extended-lambda", "--use_fast_math",
     "-diag-suppress", "177",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
 ]
 
 
 def _load(name, sources, cuda_flags, cflags=()):
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", str(os.cpu_count() or 8))
     from torch.utils.cpp_extension import load
     bdir = OUT / name
@@ -138,7 +145,7 @@ def stage_scripts():
 
 def load_prebuilt(name: str):
     """Import an already built oracle/_ref module (used on the GPU box, where
-    /root/reference does not exist).  Returns None if it was never built."""
+    no reference checkout is configured).  Returns None if it was never built."""
     import importlib.util
     so = OUT / name / f"{name}.so"
     if not so.exists():
@@ -151,8 +158,8 @@ def load_prebuilt(name: str):
 
 
 if __name__ == "__main__":
-    if not REF.exists():
-        print(f"{REF} not present: nothing to build (prebuilt oracle/_ref is used as is)")
+    if not reference_present():
+        print(f"no reference checkout at {REF} (set LEETCUDA_REFERENCE): nothing to build, a prebuilt oracle/_ref is used as is")
         sys.exit(0)
     which = sys.argv[1:] or ["hgemm", "fa", "ffpa", "sgemm", "merge", "rope", "rmsnorm", "scripts"]
     for w in which:

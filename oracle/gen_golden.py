@@ -1,8 +1,8 @@
 """TEST INFRASTRUCTURE — generate golden vectors from the reference's own kernels.
 
-Runs ON THE GPU BOX (under gpurun) with the prebuilt oracle/_ref modules (the
-UNMODIFIED reference kernels compiled for sm_100a by oracle/build_ref.py) and writes
-their outputs for seeded inputs to gpurun_out/golden/*.npz; the files are then
+Runs on a GPU machine with the prebuilt oracle/_ref modules (the
+UNMODIFIED reference kernels compiled for sm_90a by oracle/build_ref.py) and writes
+their outputs for seeded inputs to <out>/golden/*.npz (default: the system temp directory); the files are then
 committed under tests/golden/.  Inputs are NOT stored: they are regenerated from
 the numpy seed by `golden_inputs()` below (also imported by the tests), so a
 fixture is {meta, reference outputs}.
@@ -14,6 +14,7 @@ from __future__ import annotations
 import json
 import os
 import sys
+import tempfile
 from pathlib import Path
 
 import numpy as np
@@ -290,5 +291,5 @@ def main(outdir: Path, only=()):
 
 
 if __name__ == "__main__":
-    main(Path(sys.argv[1]) if len(sys.argv) > 1 else HERE.parent / "gpurun_out" / "golden",
+    main(Path(sys.argv[1]) if len(sys.argv) > 1 else Path(tempfile.gettempdir()) / "golden",
          only=tuple(sys.argv[2:]))

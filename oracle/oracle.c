@@ -11,7 +11,7 @@
  *
  *   oracle_hgemm_f64      exact products, double accumulation          -> double C ("truth")
  *   oracle_hgemm_f32acc   fp32 accumulation, k ascending, round to fp16 (what the
- *                         sm_100a kernel computes up to summation order)
+ *                         sm_90a kernel computes up to summation order)
  *   oracle_hgemm_f16acc   the reference's semantics: one HMMA.16816.F16 per k16
  *                         chunk, accumulator held in fp16 between chunks
  *                         (kernels/hgemm/mma/basic/hgemm_mma.cu:67-73 `mma...f16.f16.f16.f16`,

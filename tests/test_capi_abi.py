@@ -70,8 +70,8 @@ def test_missing_library_fails_loudly(monkeypatch, tmp_path):
         _capi.lib()
 
 
-def test_sass_is_blackwell_native(built_lib):
-    """tcgen05 / TMA opcodes are present in the shipped SASS (UTCHMMA, UTMALDG, LDTM)."""
+def test_sass_is_hopper_native(built_lib):
+    """wgmma / TMA / mbarrier opcodes are present in the shipped SASS (HGMMA, UTMALDG, SYNCS)."""
     import shutil
     import subprocess
     from leetcuda_b200 import _capi
@@ -79,6 +79,7 @@ def test_sass_is_blackwell_native(built_lib):
     if not Path(cuobjdump).exists():
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", str(_capi.LIB_PATH)], capture_output=True, text=True).stdout
-    for op in ("UTCHMMA", "UTMALDG", "LDTM", "UTCBAR"):
+    assert "sm_90a" in subprocess.run([cuobjdump, "-lelf", str(_capi.LIB_PATH)], capture_output=True, text=True).stdout
+    for op in ("HGMMA", "UTMALDG", "SYNCS"):
         assert op in sass, op
     assert "HMMA.16816" not in sass  # no legacy mma.sync path

@@ -7,6 +7,8 @@ restates kernels/rms-norm/rms_norm.cu:55-73 / :319-338).  Tolerances: rope |err|
 ~1 ulp (6e-8 relative) of evaluation error whichever way it is computed (powf + division in the reference, exp2f
 here), i.e. up to seq_len * 6e-8 rad on the fastest pair; rms_norm fp32 1e-5 relative, fp16 one fp16 ulp.
 """
+import json
+
 import numpy as np
 import pytest
 import torch
@@ -168,6 +170,7 @@ def test_rms_norm_vs_reference_golden(case):
     if not f.exists():
         pytest.skip("golden file not generated yet")
     g = np.load(f)
+    sub = json.loads(str(g["meta"]))["subsample"]
     gain = 1.25
     x32 = torch.from_numpy(rowwise_inputs(R, K, seed)).cuda()
     x16 = x32.half()
@@ -176,8 +179,8 @@ def test_rms_norm_vs_reference_golden(case):
     rms_norm.rms_norm_f16x8_pack_f32(x16, y16, gain)
     torch.cuda.synchronize()
     for name in ("rms_norm_f32", "rms_norm_f32x4"):
-        np.testing.assert_allclose(y32.cpu().numpy()[::4], g[name], rtol=1e-5, atol=1e-6, err_msg=name)
-    got16 = y16.cpu().numpy().astype(np.float32)[::4]      # the goldens keep every 4th row
+        np.testing.assert_allclose(y32.cpu().numpy()[::sub], g[name], rtol=1e-5, atol=1e-6, err_msg=name)
+    got16 = y16.cpu().numpy().astype(np.float32)[::sub]    # the goldens keep every sub-th row
     for name in ("rms_norm_f16x8_f32", "rms_norm_f16x8_pack_f32", "rms_norm_f16_f32"):      # fp32 statistics: one fp16 ulp
         np.testing.assert_allclose(got16, g[name].astype(np.float32), rtol=1e-3, atol=1e-3, err_msg=name)
     for name in ("rms_norm_f16_f16", "rms_norm_f16x2_f16", "rms_norm_f16x8_f16", "rms_norm_f16x8_pack_f16"):

@@ -7,8 +7,7 @@ import pytest
 import torch
 
 from leetcuda_b200 import ffpa_attn, flash_attn, hgemm, sgemm
-
-REF = Path("/root/reference")
+from oracle.build_ref import REF, reference_present
 
 
 def _ref_names(rel):
@@ -19,7 +18,7 @@ def _ref_names(rel):
 
 # frozen copies of the reference's bound names (kernels/hgemm/pybind/hgemm.cc:124-182,
 # kernels/flash-attn/pybind/flash_attn.cc:168-224) so the test also runs where
-# /root/reference is absent
+# no reference checkout is configured ($LEETCUDA_REFERENCE)
 HGEMM_COUNT, FA_COUNT, SGEMM_COUNT = 38, 29, 17
 
 
@@ -28,7 +27,7 @@ def test_hgemm_surface_complete():
     assert len(names) == HGEMM_COUNT
     for n in names:
         assert callable(getattr(hgemm, n))
-    if REF.exists():
+    if reference_present():
         assert set(_ref_names("kernels/hgemm/pybind/hgemm.cc")) == names
 
 
@@ -38,7 +37,7 @@ def test_sgemm_surface_complete():
     assert len(names) == SGEMM_COUNT
     for n in names:
         assert callable(getattr(sgemm, n))
-    if REF.exists():
+    if reference_present():
         assert set(_ref_names("kernels/sgemm/sgemm.cu")) == names
     s6 = inspect.signature(sgemm.sgemm_wmma_m16n16k8_mma4x2_warp2x4_stages_dsmem)
     assert list(s6.parameters) == ["a", "b", "c", "stages", "swizzle", "swizzle_stride"]
@@ -74,7 +73,7 @@ def test_flash_attn_surface_complete():
     assert len(names) == FA_COUNT
     for n in names:
         assert callable(getattr(flash_attn, n))
-    if REF.exists():
+    if reference_present():
         assert set(_ref_names("kernels/flash-attn/pybind/flash_attn.cc")) == names
 
 

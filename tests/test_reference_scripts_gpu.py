@@ -1,19 +1,20 @@
-"""The reference's own bench / test scripts, UNMODIFIED, against the sm_100a mirror (north_star: "drop-in
+"""The reference's own bench / test scripts, UNMODIFIED, against the sm_90a mirror (north_star: "drop-in
 replacements callable from the existing bench scripts"; SURVEY Appendix B).
 
 `python oracle/build_ref.py scripts` stages the scripts byte for byte under oracle/_ref/scripts/ (git-ignored,
-shipped with the gpurun snapshot; /root/reference itself does not exist on the GPU box).
+the tests skip where they have not been staged).
 tools/run_reference_script.py injects the mirror modules under the names the scripts load
 (toy_hgemm, flash_attn_lib, ffpa_attn, sgemm_lib, merge_attn_states_cuda) and runs them.  The tests assert
 on the scripts' own output: their `all close: True` lines (flash_attn_mma.py:465-494,
 test_ffpa_attn.py:583-614), the TFLOPS rows of hgemm.py:281-329, and the reference's pytest for
 merge_attn_states (test_merge_attn_states.py:95-300).  The printed tables are written to
-gpurun_out/ref_scripts_*.log (copied to profiles/ when refreshed).
+ref_scripts_*.log in the system temp directory.
 """
 import os
 import re
 import subprocess
 import sys
+import tempfile
 from pathlib import Path
 
 import pytest
@@ -29,12 +30,11 @@ def _run(rel, *args, pytest_mode=False, timeout=900, log=None):
     if not script.exists():
         pytest.skip(f"{script} not staged (python oracle/build_ref.py scripts)")
     cmd = [sys.executable, str(LAUNCH)] + (["--pytest"] if pytest_mode else []) + [str(script), *args]
-    env = dict(os.environ, PYTHONUNBUFFERED="1", TORCH_CUDA_ARCH_LIST="10.0a")
+    env = dict(os.environ, PYTHONUNBUFFERED="1", TORCH_CUDA_ARCH_LIST="9.0a")
     r = subprocess.run(cmd, capture_output=True, text=True, timeout=timeout, env=env, cwd=ROOT)
     text = r.stdout + "\n" + r.stderr[-4000:]
     if log:
-        out = ROOT / "gpurun_out"
-        out.mkdir(exist_ok=True)
+        out = Path(tempfile.gettempdir())
         (out / log).write_text("$ " + " ".join(cmd[1:]) + "\n" + r.stdout + ("\n[stderr tail]\n" + r.stderr[-2000:] if r.returncode else ""))
     assert r.returncode == 0, text[-3000:]
     return r.stdout
@@ -48,7 +48,7 @@ def test_hgemm_script_small_and_headline():
     out = _run("kernels/hgemm/hgemm.py", "--MNK", "8192", "--mma", "--mma-tn", "--cute-tn", "--wmma", "--show-all-info", "--i", "20",
                log="ref_scripts_hgemm_8192.log")
     tf = [float(x) for x in re.findall(r"TFLOPS:\s*([0-9.]+)", out)]
-    assert tf and max(tf) > 1000.0, out[-2000:]        # the script's own host-clock TFLOPS of the tcgen05 kernel
+    assert tf and max(tf) > 300.0, out[-2000:]         # the script's own host-clock TFLOPS of the wgmma kernel
 
 
 def test_flash_attn_script_check():

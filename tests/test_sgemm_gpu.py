@@ -55,7 +55,7 @@ def test_vs_oracle_small(shape, tn):
 
 
 def test_unrounded_operands_are_truncated_by_the_tensor_core():
-    """round_inputs=False leaves a, b untouched; tcgen05 kind::tf32 then reads the upper 19 bits."""
+    """round_inputs=False leaves a, b untouched; the TF32 wgmma then reads the upper 19 bits."""
     M, N, K = 256, 256, 512
     a_np, b_np = sgemm_inputs(M, N, K, seed=9)
     a, b = _dev(a_np), _dev(b_np)
@@ -72,7 +72,7 @@ def test_unrounded_operands_are_truncated_by_the_tensor_core():
 
 @pytest.mark.parametrize("case", SGEMM_CASES)
 def test_vs_reference_golden(case):
-    """Against the recorded outputs of the reference's own wmma TF32 kernels (rebuilt for sm_100a):
+    """Against the recorded outputs of the reference's own wmma TF32 kernels (rebuilt for sm_100a when they were recorded):
     same operands bit for bit, results within the accumulation-order bound, and at least as close
     to the exact product as the reference is."""
     M, N, K, seed = case
@@ -120,7 +120,7 @@ def test_every_op_name_computes_the_same_gemm():
 
 @pytest.mark.parametrize("shape", [(256, 384, 128), (1024, 1024, 1024), (512, 640, 4096), (96, 100, 36)])
 def test_3xtf32_accuracy_and_fp32_names(shape, monkeypatch):
-    """sgemm_3xtf32 (operands split into two exact TF32 numbers, one tcgen05 GEMM over K' = 3K): a and b stay untouched,
+    """sgemm_3xtf32 (operands split into two exact TF32 numbers, one wgmma GEMM over K' = 3K): a and b stay untouched,
     the error against an fp64 product is far below a plain TF32 product's and bounded by the tensor core's accumulation
     (K * 2^-23 of the largest output, the bound the TF32 tests use) — but not FFMA-grade, which is why the reference's
     fp32 op names stay vendor rows unless LEETCUDA_B200_SGEMM_FP32=3xtf32."""

@@ -1,9 +1,10 @@
-"""Side-by-side throughput table on one B200: this library vs the reference's own kernels
-(recompiled unmodified for sm_100a, oracle/_ref) vs the vendor libraries, at the BASELINE shapes.
-Writes gpurun_out/side_by_side.{json,md}; asserts only the weak claim "not slower than the
+"""Side-by-side throughput table on one H100: this library vs the reference's own kernels
+(recompiled unmodified for sm_90a, oracle/_ref, where built) vs the vendor libraries, at the BASELINE shapes.
+Writes side_by_side.{json,md} to $LEETCUDA_SIDE_BY_SIDE_DIR (default: the system temp directory); asserts only the weak claim "not slower than the
 reference kernels it replaces".  CUDA-event timing, warm-up 3, 10 iterations each."""
 import json
 import os
+import tempfile
 from pathlib import Path
 
 import pytest
@@ -14,7 +15,7 @@ from leetcuda_b200 import ffpa_attn, flash_attn, hgemm
 from oracle.build_ref import load_prebuilt
 
 pytestmark = pytest.mark.gpu
-OUT = Path(os.environ.get("GRAFT_REPO_ROOT", Path(__file__).resolve().parent.parent)) / "gpurun_out"
+OUT = Path(os.environ.get("LEETCUDA_SIDE_BY_SIDE_DIR", Path(tempfile.gettempdir()) / "leetcuda_side_by_side"))
 ROWS = []
 
 
@@ -36,7 +37,7 @@ def add(group, name, ms, flops):
 
 
 def _flush():
-    OUT.mkdir(exist_ok=True)
+    OUT.mkdir(parents=True, exist_ok=True)
     (OUT / "side_by_side.json").write_text(json.dumps(ROWS, indent=1))
     lines = ["| workload | implementation | ms | TFLOPS |", "|---|---|---:|---:|"]
     lines += [f"| {r['workload']} | {r['impl']} | {r['ms']:.4f} | {r['tflops']:.1f} |" for r in ROWS]
@@ -53,9 +54,9 @@ def test_hgemm_side_by_side(S):
     fl = 2.0 * S ** 3
     grp = f"HGEMM {S}^3 fp16"
     ours_nn = timeit(lambda: hgemm.hgemm_mma_m16n8k16_mma2x4_warp4x4x2_stages_dsmem_swizzle(a, b, c, 2, True, 2048))
-    add(grp, "leetcuda_b200 NN (tcgen05/TMA)", ours_nn, fl)
+    add(grp, "leetcuda_b200 NN (wgmma/TMA)", ours_nn, fl)
     ours_tn = timeit(lambda: hgemm.hgemm_mma_stages_block_swizzle_tn_cute(a, bt, c, 2, True, 2048))
-    add(grp, "leetcuda_b200 TN (tcgen05/TMA)", ours_tn, fl)
+    add(grp, "leetcuda_b200 TN (wgmma/TMA)", ours_tn, fl)
     add(grp, "cuBLAS NN (torch.matmul)", timeit(lambda: torch.matmul(a, b, out=c)), fl)
     ref = load_prebuilt("ref_hgemm")
     best_ref = None
@@ -68,7 +69,7 @@ def test_hgemm_side_by_side(S):
                          ("hgemm_mma_stages_block_swizzle_tn_cute", bt)]:
             for st in (2, 3):
                 ms = timeit(lambda: getattr(ref, name)(a, bb, c, st, True, stride))
-                add(grp, f"reference {name} stages={st} (sm_100a rebuild)", ms, fl)
+                add(grp, f"reference {name} stages={st} (sm_90a rebuild)", ms, fl)
                 best_ref = ms if best_ref is None else min(best_ref, ms)
         ref.init_cublas_handle()
         add(grp, "reference hgemm_cublas_tensor_op_nn (COMPUTE_16F)", timeit(lambda: ref.hgemm_cublas_tensor_op_nn(a, b, c)), fl)
@@ -86,7 +87,7 @@ def test_attention_side_by_side():
     fl = 4.0 * B * H * N * N * D
     grp = f"FA-2 fwd B{B} H{H} N{N} D{D} fp16"
     ours = timeit(lambda: flash_attn.flash_attn_mma_stages_split_q_shared_qkv(q, k, v, o, 2))
-    add(grp, "leetcuda_b200 fused tcgen05 FMHA", ours, fl)
+    add(grp, "leetcuda_b200 fused wgmma FMHA", ours, fl)
     from torch.nn.attention import SDPBackend, sdpa_kernel
     for be in (SDPBackend.CUDNN_ATTENTION, SDPBackend.FLASH_ATTENTION, SDPBackend.EFFICIENT_ATTENTION):
         try:
@@ -110,7 +111,7 @@ def test_attention_side_by_side():
                     ms = timeit(lambda: getattr(ref, name)(q, k, v, o, st), iters=5, warmup=2)
                 except Exception:
                     continue
-                add(grp, f"reference {name} stages={st} (sm_100a rebuild)", ms, fl)
+                add(grp, f"reference {name} stages={st} (sm_90a rebuild)", ms, fl)
                 best_ref = ms if best_ref is None else min(best_ref, ms)
     _flush()
     if best_ref is not None:
@@ -126,7 +127,7 @@ def test_ffpa_side_by_side():
     grp = f"FFPA fwd B{B} H{H} N{N} D{D} fp16"
     try:
         ours = timeit(lambda: ffpa_attn.ffpa_mma_acc_f32_L1(q, k, v, o, 2))
-        add(grp, "leetcuda_b200 CTA-pair tcgen05 attention (cta_group::2, M=128)", ours, fl)
+        add(grp, "leetcuda_b200 wgmma attention, 256-column slabs", ours, fl)
     except RuntimeError as e:
         ours = None
         add(grp, f"leetcuda_b200: {e}", float("nan"), fl)
@@ -145,7 +146,7 @@ def test_ffpa_side_by_side():
                     ms = timeit(lambda: getattr(ref, name)(q, k, v, o, st), iters=5, warmup=2)
                 except Exception:
                     continue
-                add(grp, f"reference {name} stages={st} (sm_100a rebuild)", ms, fl)
+                add(grp, f"reference {name} stages={st} (sm_90a rebuild)", ms, fl)
                 best_ref = ms if best_ref is None else min(best_ref, ms)
     _flush()
     if ours is not None and best_ref is not None:
@@ -164,7 +165,7 @@ def test_sgemm_tf32_side_by_side():
     fl = 2.0 * S ** 3
     grp = f"SGEMM {S}^3 fp32 (TF32 tensor cores)"
     ours = timeit(lambda: sgemm.sgemm_wmma_m16n16k8_mma4x2_warp2x4_stages(a, b, c, 2, False, 1))
-    add(grp, "leetcuda_b200 op: TF32 rounding in place + tcgen05 kind::tf32 GEMM", ours, fl)
+    add(grp, "leetcuda_b200 op: TF32 rounding in place + wgmma .tf32 GEMM", ours, fl)
     add(grp, "leetcuda_b200 GEMM kernel alone (operands already TF32)",
         timeit(lambda: sgemm.sgemm_tf32(a, b, c, round_inputs=False)), fl)
     prev = torch.backends.cuda.matmul.allow_tf32
@@ -181,7 +182,7 @@ def test_sgemm_tf32_side_by_side():
                           ("sgemm_wmma_m16n16k8_mma4x2_warp2x4_stages_dsmem", True)]:
             for st in (2, 3):
                 ms = timeit(lambda: getattr(ref, name)(a, b, c, st, swz, 1024 if swz else 1), iters=3, warmup=1)
-                add(grp, f"reference {name} stages={st}{' swizzle' if swz else ''} (sm_100a rebuild)", ms, fl)
+                add(grp, f"reference {name} stages={st}{' swizzle' if swz else ''} (sm_90a rebuild)", ms, fl)
                 best_ref = ms if best_ref is None else min(best_ref, ms)
     _flush()
     if best_ref is not None:
@@ -224,7 +225,7 @@ def test_merge_attn_states_side_by_side(T):
         return p * (pe / su).t().unsqueeze(2) + s * (se / su).t().unsqueeze(2), torch.log(su) + m
     add_bw("torch eager formula (last column: GB/s)", timeit(eager, iters=5))
     if best_ref is not None:
-        add_bw("reference merge_attn_states_cuda (sm_100a rebuild; last column: GB/s)", best_ref)
+        add_bw("reference merge_attn_states_cuda (sm_90a rebuild; last column: GB/s)", best_ref)
     _flush()
     if best_ref is not None and T >= 65536:
         # the reference kernel is already bandwidth-bound; at T = 4096 both calls are launch-bound (~11 us)

@@ -29,12 +29,10 @@ def main():
 
     # a second problem (A negated) to check that back-to-back steps do not trample each other's C
     a_shard2 = (-a_shard).contiguous()
-    modes = [("nccl", {}), ("fused", {})]                      # fused: TMA stores to every peer mapping
+    modes = [("nccl", {}), ("fused", {})]                      # fused: epilogue stores to every peer mapping
     if world > 1:
-        modes.append(("fused-direct", {"B200_FUSED_EPILOGUE": "direct"}))  # per-thread multimem.st
-        # experimental, last (a fault here must not poison the modes above): one TMA store per box through the NVLS
-        # multicast mapping
-        modes.append(("fused-mc", {"B200_FUSED_EPILOGUE": "mc"}))
+        # epilogue stores through the NVLS multicast mapping (multimem.st; peer stores where the fabric has none)
+        modes.append(("fused-direct", {"B200_FUSED_EPILOGUE": "direct"}))
     only = os.environ.get("B200_DIST_PROBE_MODES")
     if only:
         modes = [m for m in modes if m[0] in only.split(",")]

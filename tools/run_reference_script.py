@@ -1,11 +1,11 @@
-"""Run one of the reference's own bench / test scripts UNMODIFIED against the B200 kernels.
+"""Run one of the reference's own bench / test scripts UNMODIFIED against the H100 kernels.
 
     python tools/run_reference_script.py <script.py> [script args...]
     python tools/run_reference_script.py --pytest <test_file.py> [pytest args...]
 
-e.g. (here)       python tools/run_reference_script.py /root/reference/kernels/hgemm/hgemm.py --MNK 8192 --mma --i 20
+e.g.              python tools/run_reference_script.py $LEETCUDA_REFERENCE/kernels/hgemm/hgemm.py --MNK 8192 --mma --i 20
      (GPU box)    python tools/run_reference_script.py oracle/_ref/scripts/kernels/hgemm/hgemm.py --MNK 8192 --mma --i 20
-                  (oracle/build_ref.py scripts stages the unmodified scripts there; /root/reference does not travel)
+                  (oracle/build_ref.py scripts stages the unmodified scripts there)
 
 The scripts locate their extension by module name (SURVEY.md Appendix B): `toy_hgemm`, JIT
 `flash_attn_lib`, `ffpa_attn` / `pyffpa_cuda`, JIT `sgemm_lib` (kernels/sgemm/sgemm.py:11), JIT
@@ -47,7 +47,7 @@ _orig_load = ext.load
 
 def _load(name, *args, **kwargs):
     if name in MIRRORS:
-        print(f"[leetcuda_b200] serving extension '{name}' from the sm_100a mirror", flush=True)
+        print(f"[leetcuda_b200] serving extension '{name}' from the sm_90a mirror", flush=True)
         return MIRRORS[name]
     return _orig_load(name, *args, **kwargs)
 

@@ -58,16 +58,6 @@ uint64_t b200_launch_count(void);
 int b200_hgemm_f16(const void* a, const void* b, void* c, int M, int N, int K, int b_layout,
                    void* stream);
 
-/* Same as b200_hgemm_f16 with explicit tuning/debug knobs (0 = default):
- *   cta_group  1 | 2      output tile: 1 = 128x128, 2 = 128x256 (other values: B200_EINVAL)
- *   group_m    >0         m-tiles per rasterisation group
- *   max_ctas   >0         cap on the persistent grid
- *   b_lbo,b_sbo,b_kstep   wgmma descriptor byte offsets of the MN-major B operand (fp16 [K,N] layout)
- */
-int b200_hgemm_f16_ex(const void* a, const void* b, void* c, int M, int N, int K, int b_layout,
-                      int cta_group, int group_m, int max_ctas, uint32_t b_lbo, uint32_t b_sbo,
-                      uint32_t b_kstep, void* stream);
-
 /* Reference-accumulation parity mode: same as b200_hgemm_f16 but the tensor core accumulates in
  * fp16 (wgmma D format f16, one rounding per k16 instruction) exactly like the reference's
  * HMMA.16816.F16 kernels (mma/basic/hgemm_mma.cu:67-73) and its cuBLAS CUBLAS_COMPUTE_16F op
@@ -156,11 +146,6 @@ int b200_sgemm_tf32(float* a, float* b, float* c, int M, int N, int K, int b_lay
  * default and use this entry only under LEETCUDA_B200_SGEMM_FP32=3xtf32.
  * a: [M,K], b: [K,N], c: [M,N] row-major fp32; a and b are not modified.  K % 4 == 0, N % 4 == 0. */
 int b200_sgemm_3xtf32(const float* a, const float* b, float* c, int M, int N, int K, void* stream);
-
-/* b200_sgemm_tf32 without the rounding pass, with the tuning/debug knobs of b200_hgemm_f16_ex. */
-int b200_sgemm_tf32_ex(const float* a, const float* b, float* c, int M, int N, int K, int b_layout,
-                       int cta_group, int group_m, int max_ctas, uint32_t b_lbo, uint32_t b_sbo,
-                       uint32_t b_kstep, void* stream);
 
 /* x[i] <- tf32(x[i]) (round to nearest, ties away), in place, n elements; x 16-byte aligned. */
 int b200_tf32_round_inplace(float* x, size_t n, void* stream);

@@ -24,7 +24,6 @@ _lib = None
 
 _vp = ctypes.c_void_p
 _i = ctypes.c_int
-_u32 = ctypes.c_uint32
 _f = ctypes.c_float
 
 # name -> (restype, argtypes); mirrors include/leetcuda_b200.h one to one
@@ -33,7 +32,6 @@ SIGNATURES = {
     "b200_last_error": (ctypes.c_char_p, []),
     "b200_launch_count": (ctypes.c_uint64, []),
     "b200_hgemm_f16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
-    "b200_hgemm_f16_ex": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _u32, _u32, _u32, _vp]),
     "b200_hgemm_f16_acc16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200_hgemm_f16_rows": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200_hgemm_f16_rows_fused": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(ctypes.c_void_p), _i, _i, _i, _i, _i, _i, _vp]),
@@ -45,7 +43,6 @@ SIGNATURES = {
     "b200_rms_norm": (_i, [_vp, _vp, _f, _i, _i, _i, _vp]),
     "b200_sgemm_tf32": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200_sgemm_3xtf32": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
-    "b200_sgemm_tf32_ex": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _u32, _u32, _u32, _vp]),
     "b200_tf32_round_inplace": (_i, [_vp, ctypes.c_size_t, _vp]),
     "b200_merge_attn_states": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200_hgemm_f16_host": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),

@@ -42,19 +42,6 @@ def _newest_header() -> float:
     return max(h.stat().st_mtime for h in hs)
 
 
-def build_variant(name: str, defines) -> Path:
-    """Experimental side build (e.g. perf experiments): all sources with extra -D flags into
-    leetcuda_b200/lib<name>.so; select it at run time with LEETCUDA_B200_LIB."""
-    out = HERE / f"lib{name}.so"
-    cmd = [nvcc(), *[f for f in NVCC_FLAGS if f not in ("-Xptxas", "-v")], *[f"-D{d}" for d in defines],
-           "-shared", "-o", str(out), *[str(CSRC / s) for s in SOURCES], "-cudart", "static",
-           "-lpthread", "-ldl", "-lrt"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(r.stdout + r.stderr)
-    return out
-
-
 def build(force: bool = False, verbose: bool = False) -> Path:
     OBJ.mkdir(exist_ok=True)
     hdr = _newest_header()

@@ -6,10 +6,6 @@
 #include "capi_common.cuh"
 #include "attn_sm90.cuh"
 
-namespace b200 { namespace host {
-int workspace(void** out, size_t bytes);
-} }
-
 namespace {
 
 using namespace b200;

@@ -115,7 +115,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       int it = 0;
       auto next = [&](uint32_t bytes) {
         const int s = it % p.ring;
-        if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1, 11);
+        if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
         mbar_expect_tx(full(s), bytes);
         ++it;
         return s;
@@ -151,7 +151,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-  mbar_wait(qbar, 0, 12);
+  mbar_wait(qbar, 0);
 
   int it = 0;
   auto release = [&](int i) {
@@ -162,7 +162,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     float s[NS];
     wg_fence();
     for (int c = 0; c < p.nq; ++c, ++it) {
-      mbar_wait(full(it % p.ring), (it / p.ring) & 1, 13);
+      mbar_wait(full(it % p.ring), (it / p.ring) & 1);
       const uint32_t qa = sq + (w * p.nq + c) * 8192, ka = sring + (it % p.ring) * SLOT;
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
@@ -239,7 +239,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
     for (int c = 0; c < (kVT ? kBN / 64 : NDC); ++c) {
       if (c >= nvc) break;
-      mbar_wait(full(it % p.ring), (it / p.ring) & 1, 14);
+      mbar_wait(full(it % p.ring), (it / p.ring) & 1);
       const uint32_t va = sring + (it % p.ring) * SLOT;
       if constexpr (kVT) {
         // chunk c = keys 64c .. 64c+63 (K-major rows of V^T), all kDS columns

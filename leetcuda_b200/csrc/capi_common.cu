@@ -22,11 +22,11 @@ void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxe
 int sm_count() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;   // H100 SXM
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -136,7 +136,7 @@ int get_tmap(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
 }  // namespace b200
 
 extern "C" {
-int b200_version(void) { return 1000; }
+int b200_version(void) { return 2000; }
 const char* b200_last_error(void) { return b200::host::last_error_buf(); }
 uint64_t b200_launch_count(void);
 }

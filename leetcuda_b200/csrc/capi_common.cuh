@@ -44,6 +44,10 @@ struct HostPipe {
 };
 int host_pipe(HostPipe** out);
 
+// Cached device workspace of the *_host entry points (per thread and device) of at least `bytes`.
+// Growing it frees the old block, so a caller must have drained its previous use.
+int workspace(void** out, size_t bytes);
+
 // Encode (or fetch from cache) a tiled tensor map over fp16 (default) or fp32 data.
 //   rank 2: dims {d0 (contiguous), d1}, strides_bytes {s1}
 //   rank 3: dims {d0, d1, d2},          strides_bytes {s1, s2}

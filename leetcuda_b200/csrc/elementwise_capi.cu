@@ -21,23 +21,13 @@
 #include <cmath>
 
 #include "capi_common.cuh"
+#include "sm90_ptx.cuh"
 
 namespace {
 
 using b200::host::fail;
-
-__device__ __forceinline__ uint4 ld_stream(const void* p) {
-  uint4 v;
-  asm volatile("ld.global.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
-               : "l"(p));
-  return v;
-}
-__device__ __forceinline__ void st_stream(void* p, const uint4& v) {
-  asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y),
-               "r"(v.z), "r"(v.w)
-               : "memory");
-}
+using b200::ld_stream;
+using b200::st_stream;
 
 // ------------------------------------------------------------------------------------------------
 // rope: one float4 (= two pairs) per thread per step; `lanes` threads cover one row of `groups` =

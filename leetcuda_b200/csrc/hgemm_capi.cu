@@ -27,14 +27,16 @@ int launch_hgemm(const CUtensorMap& ta, const CUtensorMap& tb, const hgemm::Para
   return 0;
 }
 
-// x <- tf32(x), round-to-nearest (ties away), in place: what the reference's tf32 ops do to their
+// tf32(v): round to nearest, ties away from zero
+__device__ __forceinline__ float rna(float v) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
+  return __uint_as_float(r);
+}
+
+// x <- tf32(x) in place: what the reference's tf32 ops do to their
 // inputs before the MMAs (sgemm_wmma_tf32_stage.cu:44-60, 586-592).  HBM-bound, grid-stride, float4.
 __global__ void __launch_bounds__(256) tf32_round_inplace_kernel(float* __restrict__ x, size_t n) {
-  auto rna = [](float v) -> float {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-    return __uint_as_float(r);
-  };
   const size_t n4 = n / 4;
   float4* x4 = reinterpret_cast<float4*>(x);
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
@@ -53,11 +55,6 @@ __global__ void __launch_bounds__(256) tf32_round_inplace_kernel(float* __restri
 __global__ void __launch_bounds__(256) tf32_split3_kernel(const float* __restrict__ x, float* __restrict__ out, size_t rows,
                                                           size_t cols, size_t ld_out, size_t off0, size_t off1, size_t off2,
                                                           unsigned sel) {
-  auto rna = [](float v) -> float {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-    return __uint_as_float(r);
-  };
   const size_t c4 = cols / 4;
   const size_t total = rows * c4;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
@@ -80,11 +77,6 @@ __global__ void __launch_bounds__(256) tf32_split3_kernel(const float* __restric
 // (ld = 3K; b is not written).
 __global__ void __launch_bounds__(256) tf32_transpose_kernel(float* __restrict__ b, float* __restrict__ bt, int K, int N,
                                                              int mode) {
-  auto rna = [](float v) -> float {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-    return __uint_as_float(r);
-  };
   __shared__ float tile[32][33];
   const int n0 = blockIdx.x * 32, k0 = blockIdx.y * 32;
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
@@ -131,10 +123,8 @@ struct Fanout {           // fused all-gather targets (see hgemm::Params)
   size_t elem_offset = 0;  // offset (in elements) of this shard inside the full C buffers
 };
 
-int hgemm_impl(const void* a, const void* b, void* c, int M, int N, int K, int b_layout,
-               int tile_sel, int group_m, int max_ctas, uint32_t b_lbo, uint32_t b_sbo,
-               uint32_t b_kstep, void* stream_, const Fanout* fan = nullptr, int acc_f16 = 0,
-               bool tf32 = false) {
+int hgemm_impl(const void* a, const void* b, void* c, int M, int N, int K, int b_layout, void* stream_,
+               const Fanout* fan = nullptr, bool acc_f16 = false, bool tf32 = false) {
   // tf32: a, b, c are fp32 and b is [N,K] (the callers transpose a [K,N] operand first)
   const int esize = tf32 ? 4 : 2;
   const int bke = 128 / esize;   // elements per 128-byte swizzle row = k-block
@@ -148,22 +138,17 @@ int hgemm_impl(const void* a, const void* b, void* c, int M, int N, int K, int b
   if (tf32 && b_layout != B200_B_ROW_MAJOR_NK) return fail(B200_EINVAL, "gemm: internal error (tf32 B must be [N,K])");
   if ((reinterpret_cast<uintptr_t>(c) & 15u) != 0)
     return fail(B200_EINVAL, "hgemm: c is not 16-byte aligned");
-  if (tile_sel < 0 || tile_sel > 2) return fail(B200_EINVAL, "hgemm: tile selector %d (0 auto, 1: 128x128, 2: 128x256)", tile_sel);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int sms = host::sm_count();
 
   // Tile: 128x256 (least operand traffic per flop) unless a 128x128 tiling fills the last wave of the
   // SMs markedly better (mid-size problems would otherwise leave many of the SMs idle).
-  int bn = 256;
-  if (tile_sel == 1) bn = 128;
-  if (tile_sel == 0) {
-    auto score = [&](int bnc, double eff) {
-      const long tiles = static_cast<long>((M + 127) / 128) * ((N + bnc - 1) / bnc);
-      const long waves = (tiles + sms - 1) / sms;
-      return eff * static_cast<double>(tiles) / static_cast<double>(waves * sms);
-    };
-    if (score(128, 0.90) > score(256, 1.0)) bn = 128;
-  }
+  auto score = [&](int bnc, double eff) {
+    const long tiles = static_cast<long>((M + 127) / 128) * ((N + bnc - 1) / bnc);
+    const long waves = (tiles + sms - 1) / sms;
+    return eff * static_cast<double>(tiles) / static_cast<double>(waves * sms);
+  };
+  const int bn = score(128, 0.90) > score(256, 1.0) ? 128 : 256;
 
   hgemm::Params p;
   memset(&p, 0, sizeof(p));
@@ -172,30 +157,6 @@ int hgemm_impl(const void* a, const void* b, void* c, int M, int N, int K, int b
   p.tiles_m = (M + hgemm::BM - 1) / hgemm::BM;
   p.tiles_n = (N + bn - 1) / bn;
   p.num_tiles = p.tiles_m * p.tiles_n;
-  p.group_m = group_m > 0 ? group_m : 16;
-  {
-    static int serp = -1;   // B200_HGEMM_SERPENTINE=0|1 (A/B knob), default on
-    if (serp < 0) { const char* e = getenv("B200_HGEMM_SERPENTINE"); serp = (e && e[0] == '0') ? 0 : 1; }
-    p.serpentine = serp;
-  }
-  // MN-major B (the [K,N] layout, fp16): boxes {64 n x 64 k}, 8-k-row swizzle atoms (SBO 1024), the
-  // 64-column boxes of one stage 8 KiB apart (LBO), +16 k-rows per k16 step.
-  p.b_lbo = b_lbo ? b_lbo : 8192u;
-  p.b_sbo = b_sbo ? b_sbo : 1024u;
-  p.b_kstep = b_kstep ? b_kstep : 2048u;
-  {
-    // L2 eviction priority of the A / B operand loads: A panels (re-used by the other column tiles of
-    // the same row group) evict-last, B panels normal.  B200_HGEMM_HINTS=<a><b>, each n|f|l, overrides.
-    static unsigned long long ha = 0, hb = 0;
-    if (ha == 0) {
-      auto dec = [](char ch) { return ch == 'f' ? b200::kEvictFirst : (ch == 'l' ? b200::kEvictLast : b200::kEvictNormal); };
-      const char* e = getenv("B200_HGEMM_HINTS");
-      ha = dec(e && e[0] ? e[0] : 'l');
-      hb = dec(e && e[0] && e[1] ? e[1] : 'n');
-    }
-    p.hint_a = ha;
-    p.hint_b = hb;
-  }
   if (fan) {
     if (fan->n_peers < 0 || fan->n_peers > 7) return fail(B200_EINVAL, "hgemm: %d peers", fan->n_peers);
     if (fan->mc) p.C_mc = static_cast<char*>(fan->mc) + fan->elem_offset * esize;
@@ -228,9 +189,7 @@ int hgemm_impl(const void* a, const void* b, void* c, int M, int N, int K, int b
     if (rc) return rc;
   }
 
-  int grid = p.num_tiles;
-  const int cap = (max_ctas > 0 && max_ctas < sms) ? max_ctas : sms;
-  if (grid > cap) grid = cap;
+  const int grid = p.num_tiles < sms ? p.num_tiles : sms;
 
   const bool mn = (b_layout == B200_B_ROW_MAJOR_KN);
   if (tf32)
@@ -286,26 +245,19 @@ extern "C" {
 
 int b200_hgemm_f16(const void* a, const void* b, void* c, int M, int N, int K, int b_layout,
                    void* stream) {
-  return hgemm_impl(a, b, c, M, N, K, b_layout, 0, 0, 0, 0, 0, 0, stream);
-}
-
-int b200_hgemm_f16_ex(const void* a, const void* b, void* c, int M, int N, int K, int b_layout,
-                      int cta_group, int group_m, int max_ctas, uint32_t b_lbo, uint32_t b_sbo,
-                      uint32_t b_kstep, void* stream) {
-  return hgemm_impl(a, b, c, M, N, K, b_layout, cta_group, group_m, max_ctas, b_lbo, b_sbo,
-                    b_kstep, stream);
+  return hgemm_impl(a, b, c, M, N, K, b_layout, stream);
 }
 
 int b200_hgemm_f16_acc16(const void* a, const void* b, void* c, int M, int N, int K, int b_layout,
                          void* stream) {
-  return hgemm_impl(a, b, c, M, N, K, b_layout, 0, 0, 0, 0, 0, 0, stream, nullptr, 1);
+  return hgemm_impl(a, b, c, M, N, K, b_layout, stream, nullptr, true);
 }
 
 int b200_hgemm_f16_rows(const void* a_shard, const void* b, void* c_full, int rows, int N, int K,
                         int b_layout, int row0, void* stream) {
   if (row0 < 0) return fail(B200_EINVAL, "hgemm_rows: row0 %d", row0);
   __half* c = static_cast<__half*>(c_full) + static_cast<size_t>(row0) * N;
-  return hgemm_impl(a_shard, b, c, rows, N, K, b_layout, 0, 0, 0, 0, 0, 0, stream);
+  return hgemm_impl(a_shard, b, c, rows, N, K, b_layout, stream);
 }
 
 int b200_hgemm_f16_rows_fused(const void* a_shard, const void* b, void* c_full, void* c_full_multicast,
@@ -329,7 +281,7 @@ int b200_hgemm_f16_rows_fused(const void* a_shard, const void* b, void* c_full, 
     fan.n_peers = n_peers;
   }
   __half* c = static_cast<__half*>(c_full) + fan.elem_offset;
-  return hgemm_impl(a_shard, b, c, rows, N, K, b_layout, 0, 0, 0, 0, 0, 0, stream, &fan);
+  return hgemm_impl(a_shard, b, c, rows, N, K, b_layout, stream, &fan);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -351,11 +303,8 @@ int b200_tf32_round_inplace(float* x, size_t n, void* stream_) {
   return 0;
 }
 
-}  // extern "C"
-
-namespace {
-int sgemm_tf32_impl(float* a, float* b, float* c, int M, int N, int K, int b_layout, int round, int tile_sel,
-                    int group_m, int max_ctas, void* stream_) {
+int b200_sgemm_tf32(float* a, float* b, float* c, int M, int N, int K, int b_layout,
+                    int round_inputs_in_place, void* stream_) {
   // validate everything the GEMM would reject BEFORE touching the caller's a and b
   if (!a || !b || !c || M <= 0 || N <= 0 || K <= 0) return fail(B200_EINVAL, "sgemm: bad args");
   if ((K % 4) != 0 || (N % 4) != 0)
@@ -365,28 +314,20 @@ int sgemm_tf32_impl(float* a, float* b, float* c, int M, int N, int K, int b_lay
   if (((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15u) != 0)
     return fail(B200_EINVAL, "sgemm: a, b, c must be 16-byte aligned");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const bool round = round_inputs_in_place != 0;
   int rc;
   if (round && (rc = b200_tf32_round_inplace(a, static_cast<size_t>(M) * K, stream))) return rc;
   if (b_layout == B200_B_ROW_MAJOR_NK) {
     if (round && (rc = b200_tf32_round_inplace(b, static_cast<size_t>(K) * N, stream))) return rc;
-    return hgemm_impl(a, b, c, M, N, K, B200_B_ROW_MAJOR_NK, tile_sel, group_m, max_ctas, 0, 0, 0, stream, nullptr, 0, true);
+    return hgemm_impl(a, b, c, M, N, K, B200_B_ROW_MAJOR_NK, stream, nullptr, false, true);
   }
   // [K,N]: round b in place (if asked) and transpose it into stream-ordered scratch in one pass
   float* bt = nullptr;
   B200_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&bt), static_cast<size_t>(K) * N * sizeof(float), stream));
   rc = launch_tf32_transpose(b, bt, K, N, round ? 1 : 0, stream);
-  if (!rc)
-    rc = hgemm_impl(a, bt, c, M, N, K, B200_B_ROW_MAJOR_NK, tile_sel, group_m, max_ctas, 0, 0, 0, stream, nullptr, 0, true);
+  if (!rc) rc = hgemm_impl(a, bt, c, M, N, K, B200_B_ROW_MAJOR_NK, stream, nullptr, false, true);
   cudaFreeAsync(bt, stream);
   return rc;
-}
-}  // namespace
-
-extern "C" {
-
-int b200_sgemm_tf32(float* a, float* b, float* c, int M, int N, int K, int b_layout,
-                    int round_inputs_in_place, void* stream) {
-  return sgemm_tf32_impl(a, b, c, M, N, K, b_layout, round_inputs_in_place, 0, 0, 0, stream);
 }
 
 int b200_sgemm_3xtf32(const float* a, const float* b, float* c, int M, int N, int K, void* stream_) {
@@ -411,18 +352,10 @@ int b200_sgemm_3xtf32(const float* a, const float* b, float* c, int M, int N, in
   else {
     host::count_launch();
     rc = launch_tf32_transpose(b, b3, K, N, 2, stream);                                                   // hi ; lo ; hi
-    if (!rc) rc = hgemm_impl(a3, b3, c, M, N, 3 * K, B200_B_ROW_MAJOR_NK, 0, 0, 0, 0, 0, 0, stream, nullptr, 0, true);
+    if (!rc) rc = hgemm_impl(a3, b3, c, M, N, 3 * K, B200_B_ROW_MAJOR_NK, stream, nullptr, false, true);
   }
   cudaFreeAsync(ws, stream);
   return rc;
-}
-
-int b200_sgemm_tf32_ex(const float* a, const float* b, float* c, int M, int N, int K, int b_layout,
-                       int cta_group, int group_m, int max_ctas, uint32_t b_lbo, uint32_t b_sbo,
-                       uint32_t b_kstep, void* stream) {
-  (void)b_lbo; (void)b_sbo; (void)b_kstep;   // descriptor knobs of the fp16 MN-major B operand only
-  return sgemm_tf32_impl(const_cast<float*>(a), const_cast<float*>(b), c, M, N, K, b_layout, 0, cta_group, group_m,
-                         max_ctas, stream);
 }
 
 int b200_hgemm_f16_host(const void* a, const void* b, void* c, int M, int N, int K, int b_layout,
@@ -468,7 +401,7 @@ int b200_hgemm_f16_host(const void* a, const void* b, void* c, int M, int N, int
     B200_CUDA_OK(cudaEventRecord(pipe.ev[2 * np], pipe.in));
     B200_CUDA_OK(cudaStreamWaitEvent(stream, pipe.ev[2 * np], 0));
     rc = hgemm_impl(da + static_cast<size_t>(r0) * K * 2, db, dc + static_cast<size_t>(r0) * N * 2, rows, N, K,
-                    b_layout, 0, 0, 0, 0, 0, 0, stream);
+                    b_layout, stream);
     if (rc) return rc;
     B200_CUDA_OK(cudaEventRecord(pipe.ev[2 * np + 1], stream));
     B200_CUDA_OK(cudaStreamWaitEvent(pipe.out, pipe.ev[2 * np + 1], 0));

@@ -32,6 +32,20 @@ namespace hgemm {
 constexpr int BM = 128;        // rows per tile: two consumer warpgroups x 64
 constexpr int kThreads = 384;  // three warpgroups
 
+// Rasterisation: tiles are walked in groups of kGroupM m-tiles, and odd groups walk the n-tiles backwards,
+// so a group starts on the B panels the previous group loaded last (still in L2).
+constexpr int kGroupM = 16;
+// L2 eviction priority of the operand loads: A panels (re-used by the other column tiles of the same row
+// group) evict-last, B panels normal.
+constexpr uint64_t kHintA = kEvictLast;
+constexpr uint64_t kHintB = kEvictNormal;
+// wgmma descriptor of the MN-major B operand (the fp16 [K,N] layout), which follows from its TMA boxes
+// {64 n x 64 k} with 128B swizzle: the kBN / 64 boxes of one stage lie 8 KiB apart (LBO), a swizzle atom
+// spans 8 k-rows (SBO 1 KiB), and a k16 step advances 16 k-rows (2 KiB).
+constexpr uint32_t kBLbo = 8192;
+constexpr uint32_t kBSbo = 1024;
+constexpr uint32_t kBKStep = 2048;
+
 template <int kBN>
 struct Cfg {
   static constexpr int A_BYTES = BM * 128;     // 16 KiB: 128 rows x 128 bytes of k
@@ -47,12 +61,7 @@ struct Params {
   int M, N, K;
   int ldc;
   int tiles_m, tiles_n;    // in units of BM x kBN
-  int group_m;             // rasterisation: m-tiles per L2 group
-  int serpentine;          // odd groups walk the n-tiles backwards (reuses the last B panels in L2)
   int num_tiles;
-  unsigned long long hint_a, hint_b;   // L2 cache-policy descriptors of the A / B TMA loads
-  // wgmma descriptor fields of the MN-major B operand (bytes)
-  uint32_t b_lbo, b_sbo, b_kstep;
   // Fused all-gather of C (multi-GPU row sharding, SURVEY §8e): the epilogue stores every value
   // either through an NVLS multicast mapping (one multimem.st reaches the C buffer of every GPU,
   // this one included) or to C and to each peer-mapped C buffer.  All null/0 = C only.
@@ -62,14 +71,14 @@ struct Params {
 };
 
 __device__ __forceinline__ void tile_coords(const Params& p, int t, int& tm, int& tn) {
-  const int per_group = p.group_m * p.tiles_n;
+  const int per_group = kGroupM * p.tiles_n;
   const int g = t / per_group;
   const int r = t - g * per_group;
-  const int first_m = g * p.group_m;
-  const int gm = min(p.group_m, p.tiles_m - first_m);
+  const int first_m = g * kGroupM;
+  const int gm = min(kGroupM, p.tiles_m - first_m);
   tn = r / gm;
   tm = first_m + (r - tn * gm);
-  if (p.serpentine && (g & 1)) tn = p.tiles_n - 1 - tn;
+  if (g & 1) tn = p.tiles_n - 1 - tn;
 }
 
 template <typename T>
@@ -95,10 +104,12 @@ __device__ __forceinline__ void store_pair(const Params& p, size_t off, T v) {
 // kBMn: B is [K,N] (MN-major operand; fp16 only).  kTf32: fp32 operands through wgmma .tf32 (K-major
 // A and B; a 128-byte row holds 32 elements: k-block 32, k-step 8).  kAcc16: fp16 accumulation
 // (the reference's HMMA.F16 numerics, see b200_hgemm_f16_acc16).
+// p is __grid_constant__ because the epilogue indexes p.C_peer at run time: a plain by-value struct of up to
+// 128 bytes is then copied to local memory, a __grid_constant__ one is read in place from the parameter bank.
 template <int kBN, bool kBMn, bool kTf32, bool kAcc16>
 __global__ void __launch_bounds__(kThreads, 1)
 hgemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                   const Params p) {
+                   const __grid_constant__ Params p) {
   static_assert(!(kTf32 && (kBMn || kAcc16)), "tf32 operands are K-major with fp32 accumulation");
   using C_ = Cfg<kBN>;
   constexpr int STAGES = C_::STAGES;
@@ -136,16 +147,16 @@ hgemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         const int m0 = tm * BM, n0 = tn * kBN;
         for (int kb = 0; kb < kblocks; ++kb, ++it) {
           const int s = it % STAGES;
-          if (it >= STAGES) mbar_wait(empty(s), ((it / STAGES) - 1) & 1, 1);
+          if (it >= STAGES) mbar_wait(empty(s), ((it / STAGES) - 1) & 1);
           const uint32_t sa = sbase + s * C_::STAGE_BYTES, sb = sa + C_::A_BYTES;
           mbar_expect_tx(full(s), C_::STAGE_BYTES);
-          tma_load_2d(sa, &tmap_a, full(s), kb * BKE, m0, p.hint_a);
+          tma_load_2d(sa, &tmap_a, full(s), kb * BKE, m0, kHintA);
           if constexpr (kBMn) {
 #pragma unroll
             for (int c = 0; c < kBN / 64; ++c)
-              tma_load_2d(sb + c * 8192, &tmap_b, full(s), n0 + 64 * c, kb * 64, p.hint_b);
+              tma_load_2d(sb + c * kBLbo, &tmap_b, full(s), n0 + 64 * c, kb * 64, kHintB);
           } else {
-            tma_load_2d(sb, &tmap_b, full(s), kb * BKE, n0, p.hint_b);
+            tma_load_2d(sb, &tmap_b, full(s), kb * BKE, n0, kHintB);
           }
         }
       }
@@ -166,7 +177,7 @@ hgemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     for (int i = 0; i < NACC; ++i) acc[i] = 0;
     for (int kb = 0; kb < kblocks; ++kb, ++it) {
       const int s = it % STAGES;
-      mbar_wait(full(s), (it / STAGES) & 1, 2);
+      mbar_wait(full(s), (it / STAGES) & 1);
       const uint32_t sa = sbase + s * C_::STAGE_BYTES + (wg - 1) * 64 * 128, sb = sbase + s * C_::STAGE_BYTES + C_::A_BYTES;
       wg_fence();
 #pragma unroll
@@ -178,7 +189,7 @@ hgemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           if constexpr (kBN == 256) wgmma_ss_m64n256k8_f32_tf32(acc, da, db, go);
           else wgmma_ss_m64n128k8_f32_tf32(acc, da, db, go);
         } else {
-          const uint64_t db = kBMn ? wg_desc(sb + ks * p.b_kstep, p.b_lbo, p.b_sbo) : wg_desc(sb + ks * 32, 16);
+          const uint64_t db = kBMn ? wg_desc(sb + ks * kBKStep, kBLbo, kBSbo) : wg_desc(sb + ks * 32, 16);
           constexpr int kTB = kBMn ? 1 : 0;
           if constexpr (kAcc16 && kBN == 256) wgmma_ss_m64n256k16_f16_f16<0, kTB>(acc, da, db, go);
           else if constexpr (kAcc16) wgmma_ss_m64n128k16_f16_f16<0, kTB>(acc, da, db, go);

@@ -9,13 +9,10 @@
 //
 // HBM-bound element-wise work: 3 * D * sizeof(T) + 12 bytes per (token, head) row.
 //
-// Layout: one thread per 16-byte pack of the output, ONE-SHOT grid (packs / 256 CTAs of 256 threads, 32-bit index
+// Layout: one thread per 16-byte pack of the output, one-shot grid (packs / 256 CTAs of 256 threads, 32-bit index
 // arithmetic whenever the pack count fits): both 128-bit L1-bypassing loads of a pack are issued before the two
 // lse values are fetched.  Every thread of a row evaluates the row's two weights itself (a warp executes those few
-// instructions once for all its lanes either way).  On the B200 this was first written for, that layout beat a
-// persistent grid-stride loop, plain (cached) accesses and a row-per-lane-group layout; not re-measured on H100.
-// i.e. for this two-reads-one-write stream the hardware's block scheduler spreads the three address streams
-// better than a lock-step grid-stride loop, and the kernel lives off independent threads, not instruction count.
+// instructions once for all its lanes either way).
 //
 // Numerics: libdevice expf / logf, IEEE division, and per element one multiply and one fused
 // multiply-add in fp32 — the operations (not the code) of the reference's kernel, so the outputs
@@ -26,30 +23,14 @@
 #include <cmath>
 #include <limits>
 
-#include <stdlib.h>
-
 #include "capi_common.cuh"
-
-#ifndef B200_MERGE_VARIANT_DEFAULT
-#define B200_MERGE_VARIANT_DEFAULT 1
-#endif
+#include "sm90_ptx.cuh"
 
 namespace {
 
 using b200::host::fail;
-
-__device__ __forceinline__ uint4 ld_stream(const void* p) {
-  uint4 v;
-  asm volatile("ld.global.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
-               : "l"(p));
-  return v;
-}
-__device__ __forceinline__ void st_stream(void* p, const uint4& v) {
-  asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y),
-               "r"(v.z), "r"(v.w)
-               : "memory");
-}
+using b200::ld_stream;
+using b200::st_stream;
 
 // one 16-byte pack: out = prefix * wp + suffix * ws, element type T, arithmetic in fp32
 template <typename T>
@@ -94,10 +75,9 @@ struct Pack<__nv_bfloat16> {
   }
 };
 
-// Idx: 32-bit pack indices whenever they fit (64-bit division is emulated).
-// kStream: L1-bypassing 128-bit loads/stores (else plain ld/st.global).  The grid is either persistent (grid-stride) or
-// one-shot (one pack per thread, gridDim = packs / 256) — the loop below covers both.
-template <typename T, typename Idx, bool kStream>
+// Idx: 32-bit pack indices whenever they fit (64-bit division is emulated).  The grid has one thread per pack, so the
+// grid-stride loop runs its body at most once per thread.
+template <typename T, typename Idx>
 __global__ void __launch_bounds__(256)
 merge_attn_states_kernel(T* __restrict__ out, float* __restrict__ out_lse, const T* __restrict__ prefix,
                          const float* __restrict__ prefix_lse, const T* __restrict__ suffix,
@@ -107,8 +87,8 @@ merge_attn_states_kernel(T* __restrict__ out, float* __restrict__ out_lse, const
   const Idx step = static_cast<Idx>(gridDim.x) * blockDim.x;
   for (Idx pk = static_cast<Idx>(blockIdx.x) * blockDim.x + threadIdx.x; pk < n_packs; pk += step) {
     // the two data packs first: they are the long-latency part
-    const uint4 a = kStream ? ld_stream(reinterpret_cast<const uint4*>(prefix) + pk) : reinterpret_cast<const uint4*>(prefix)[pk];
-    const uint4 b = kStream ? ld_stream(reinterpret_cast<const uint4*>(suffix) + pk) : reinterpret_cast<const uint4*>(suffix)[pk];
+    const uint4 a = ld_stream(reinterpret_cast<const uint4*>(prefix) + pk);
+    const uint4 b = ld_stream(reinterpret_cast<const uint4*>(suffix) + pk);
     const Idx row = pk / packs_per_row;                              // = token * num_heads + head
     const unsigned token = static_cast<unsigned>(row / num_heads);
     const unsigned head = static_cast<unsigned>(row - static_cast<Idx>(token) * num_heads);
@@ -120,8 +100,7 @@ merge_attn_states_kernel(T* __restrict__ out, float* __restrict__ out_lse, const
     const float ep = expf(lp - top), es = expf(ls - top);
     const float denom = ep + es;
     const uint4 r = Pack<T>::blend(a, b, ep / denom, es / denom);
-    if (kStream) st_stream(reinterpret_cast<uint4*>(out) + pk, r);
-    else reinterpret_cast<uint4*>(out)[pk] = r;
+    st_stream(reinterpret_cast<uint4*>(out) + pk, r);
     if (out_lse != nullptr && pk == row * packs_per_row) out_lse[at] = logf(denom) + top;   // first pack of the row
   }
 }
@@ -134,17 +113,7 @@ int launch_merge(void* out, float* out_lse, const void* prefix, const float* pre
     return fail(B200_EINVAL, "headsize must be multiple of pack_size:%d", kPack);   // reference :131-132
   const unsigned packs = static_cast<unsigned>(head_size / kPack);
   const size_t total = static_cast<size_t>(num_tokens) * num_heads * packs;
-  // B200_MERGE_VARIANT (A/B knob): 0 = persistent grid + streaming accesses, 1 = one-shot grid + streaming accesses,
-  // 2 = one-shot grid + plain accesses (the reference's launch shape)
-  static int variant = -1;
-  if (variant < 0) {
-    const char* e = getenv("B200_MERGE_VARIANT");
-    variant = (e && e[0] >= '0' && e[0] <= '2') ? (e[0] - '0') : B200_MERGE_VARIANT_DEFAULT;
-  }
-  size_t blocks = (total + 255) / 256;
-  const size_t cap = static_cast<size_t>(b200::host::sm_count()) * 8;      // 8 x 256 threads resident per SM
-  if (variant == 0 && blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  const size_t blocks = (total + 255) / 256;
   if (blocks > 0x7FFFFFFFull) return fail(B200_EINVAL, "merge_attn_states: too many packs");
   const unsigned g = static_cast<unsigned>(blocks);
   T* o = static_cast<T*>(out);
@@ -153,13 +122,8 @@ int launch_merge(void* out, float* out_lse, const void* prefix, const float* pre
   const unsigned nt = static_cast<unsigned>(num_tokens), nh = static_cast<unsigned>(num_heads);
   // the grid-stride loop adds up to one stride past `total`: keep that inside 32 bits too
   const bool idx32 = total + blocks * 256 < 0xFFFFFFFFull;
-  if (variant == 2) {
-    if (idx32) merge_attn_states_kernel<T, unsigned, false><<<g, 256, 0, stream>>>(o, out_lse, pa, prefix_lse, pb, suffix_lse, nt, nh, packs);
-    else merge_attn_states_kernel<T, size_t, false><<<g, 256, 0, stream>>>(o, out_lse, pa, prefix_lse, pb, suffix_lse, nt, nh, packs);
-  } else {
-    if (idx32) merge_attn_states_kernel<T, unsigned, true><<<g, 256, 0, stream>>>(o, out_lse, pa, prefix_lse, pb, suffix_lse, nt, nh, packs);
-    else merge_attn_states_kernel<T, size_t, true><<<g, 256, 0, stream>>>(o, out_lse, pa, prefix_lse, pb, suffix_lse, nt, nh, packs);
-  }
+  if (idx32) merge_attn_states_kernel<T, unsigned><<<g, 256, 0, stream>>>(o, out_lse, pa, prefix_lse, pb, suffix_lse, nt, nh, packs);
+  else merge_attn_states_kernel<T, size_t><<<g, 256, 0, stream>>>(o, out_lse, pa, prefix_lse, pb, suffix_lse, nt, nh, packs);
   B200_CUDA_OK(cudaGetLastError());
   b200::host::count_launch();
   return 0;

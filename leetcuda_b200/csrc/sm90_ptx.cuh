@@ -8,7 +8,6 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 namespace b200 {
 
@@ -20,20 +19,6 @@ namespace b200 {
 B200_DEVICE uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-B200_DEVICE bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-B200_DEVICE uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
 B200_DEVICE void cluster_arrive() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
 }
@@ -43,9 +28,6 @@ B200_DEVICE void cluster_wait() {
 B200_DEVICE void cluster_sync_all() {
   cluster_arrive();
   cluster_wait();
-}
-B200_DEVICE void named_bar_sync(uint32_t id, uint32_t nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 template <int N>
 B200_DEVICE void reg_dealloc() {
@@ -66,25 +48,12 @@ B200_DEVICE void fence_mbar_init() {
   // make mbarrier inits visible to the async proxy / other CTAs of the cluster
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-B200_DEVICE void fence_proxy_async_smem() {
-  // generic-proxy smem writes -> visible to async proxy (TMA store, wgmma reads)
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
 B200_DEVICE void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes)
                : "memory");
 }
 B200_DEVICE void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `cta` of the cluster
-B200_DEVICE void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}\n" ::"r"(bar),
-      "r"(cta)
-      : "memory");
 }
 B200_DEVICE bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
@@ -108,38 +77,13 @@ B200_DEVICE bool mbar_try_wait(uint32_t bar, uint32_t parity) {
 #define B200_WATCHDOG_CYCLES 20000000000ll
 #endif
 
-B200_DEVICE void mbar_watchdog(long long t0, int tag, uint32_t parity) {
-  (void)tag;
-  (void)parity;
+B200_DEVICE void mbar_wait(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
 #if B200_WATCHDOG_CYCLES > 0
-  if (clock64() - t0 > B200_WATCHDOG_CYCLES) __trap();
+    if (clock64() - t0 > B200_WATCHDOG_CYCLES) __trap();
 #endif
-}
-
-B200_DEVICE void mbar_wait(uint32_t bar, uint32_t parity, int tag = 0) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) mbar_watchdog(t0, tag, parity);
-}
-
-// Same wait, but a failed poll suspends the warp until the barrier is signalled (or kHintNs
-// elapse): NANOSLEEP.SYNCS in SASS instead of a spinning TRYWAIT/BRA loop.  For waits with
-// slack (GEMM pipeline roles run several stages ahead) the wake-up latency does not matter.
-template <uint32_t kHintNs>
-B200_DEVICE void mbar_wait_suspend(uint32_t bar, uint32_t parity, int tag = 0) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred P;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, P;\n\t}\n"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity), "r"(kHintNs)
-        : "memory");
-    if (ok) return;
-    mbar_watchdog(t0, tag, parity);
   }
 }
 
@@ -169,28 +113,6 @@ B200_DEVICE void tma_load_3d(uint32_t dst, const void* tmap, uint32_t bar, int c
       " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(dst),
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "l"(hint)
       : "memory");
-}
-B200_DEVICE void tma_store_2d(const void* tmap, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tmap)),
-               "r"(src), "r"(c0), "r"(c1)
-               : "memory");
-}
-B200_DEVICE void tma_store_3d(const void* tmap, uint32_t src, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-          reinterpret_cast<uint64_t>(tmap)),
-      "r"(src), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-B200_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-B200_DEVICE void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-B200_DEVICE void tma_store_wait() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 // map a local smem address into the cluster window of CTA `cta`
 B200_DEVICE uint32_t mapa(uint32_t addr, uint32_t cta) {
@@ -327,23 +249,19 @@ B200_DEVICE void wgmma_rs_m64n64k16_f32_f16(float (&d)[32], const uint32_t (&a)[
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc), "n"(kTransB));
 }
 
-template <int kTransB>
-B200_DEVICE void wgmma_rs_m64n128k16_f32_f16(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "{%64, %65, %66, %67}, %68, p, 1, 1, %70;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc), "n"(kTransB));
+// ----------------------------------------------------------------------------
+// streaming global memory: 128-bit accesses that bypass L1
+// ----------------------------------------------------------------------------
+B200_DEVICE uint4 ld_stream(const void* p) {
+  uint4 v;
+  asm volatile("ld.global.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+               : "l"(p));
+  return v;
 }
-
-// 16-byte store through an NVLS multicast mapping: the NVSwitch replicates it into the
-// memory of every GPU bound to the multicast object.
-B200_DEVICE void st_multicast_v4(void* mc_addr, const uint4& v) {
-  asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(mc_addr),
-               "f"(__uint_as_float(v.x)), "f"(__uint_as_float(v.y)), "f"(__uint_as_float(v.z)),
-               "f"(__uint_as_float(v.w))
+B200_DEVICE void st_stream(void* p, const uint4& v) {
+  asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y),
+               "r"(v.z), "r"(v.w)
                : "memory");
 }
 
@@ -355,13 +273,9 @@ B200_DEVICE uint32_t pack_half2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 B200_DEVICE float fast_exp2(float x) {
-#ifdef B200_EXPERIMENT_FAKE_EXP
-  return x * x;   // perf experiment only (wrong results): how fast is the kernel without MUFU?
-#else
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));   // pure: let the scheduler interleave it
   return y;
-#endif
 }
 
 }  // namespace b200

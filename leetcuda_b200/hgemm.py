@@ -116,22 +116,6 @@ def hgemm(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, *, tn: bool = False
     _capi.check(rc, "hgemm")
 
 
-def hgemm_ex(a, b, c, *, tn=False, cta_group=0, group_m=0, max_ctas=0, b_lbo=0, b_sbo=0,
-             b_kstep=0) -> None:
-    """Same as :func:`hgemm` with the tuning/debug knobs of ``b200_hgemm_f16_ex``."""
-    _check_half(a); _check_half(b); _check_half(c)
-    M, K = a.size(0), a.size(1)
-    N = b.size(1)
-    _check_shape(b, K, N)
-    _check_shape(c, M, N)
-    rc = _capi.lib().b200_hgemm_f16_ex(
-        a.data_ptr(), b.data_ptr(), c.data_ptr(), M, N, K,
-        _capi.B_ROW_MAJOR_NK if tn else _capi.B_ROW_MAJOR_KN,
-        cta_group, group_m, max_ctas, b_lbo, b_sbo, b_kstep,
-        torch.cuda.current_stream(a.device).cuda_stream)
-    _capi.check(rc, "hgemm_ex")
-
-
 def hgemm_host(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, *, tn: bool = False) -> None:
     """Host-buffer entry point (``b200_hgemm_f16_host``): ``a``, ``b``, ``c`` are CPU tensors
     (pinned for full PCIe rate).  Copies in, multiplies on the current device and copies out,
@@ -205,5 +189,5 @@ def destroy_cublas_handle() -> None:
     """reference: cublas/hgemm_cublas.cu:27-38 (no-op here)."""
 
 
-__all__ = OP_NAMES + ["init_cublas_handle", "destroy_cublas_handle", "hgemm", "hgemm_ex", "hgemm_host",
+__all__ = OP_NAMES + ["init_cublas_handle", "destroy_cublas_handle", "hgemm", "hgemm_host",
                       "OP_NAMES"]

@@ -39,7 +39,7 @@ _OPS_CUBLAS = ["sgemm_cublas", "sgemm_cublas_tf32"]
 _OPS_TF32_STAGED = ["sgemm_wmma_m16n16k8_mma4x2_warp2x4_stages",
                     "sgemm_wmma_m16n16k8_mma4x2_warp2x4_stages_dsmem"]
 OP_NAMES = _OPS_FP32_CUDA_CORE + _OPS_CUBLAS + _OPS_TF32_STAGED
-__all__ = OP_NAMES + ["sgemm_tf32", "sgemm_tf32_ex", "sgemm_3xtf32", "tf32_round_", "OP_NAMES"]
+__all__ = OP_NAMES + ["sgemm_tf32", "sgemm_3xtf32", "tf32_round_", "OP_NAMES"]
 
 
 def _check_f32(t: torch.Tensor) -> None:
@@ -92,19 +92,6 @@ def sgemm_tf32(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, *, tn: bool = 
         rc = fn(a.data_ptr(), b.data_ptr(), c.data_ptr(), M, N, K, layout, int(round_inputs),
                 _capi.raw_stream(idx))
     _capi.check(rc, "sgemm_tf32")
-
-
-def sgemm_tf32_ex(a, b, c, *, tn=False, cta_group=0, group_m=0, max_ctas=0, b_lbo=0, b_sbo=0,
-                  b_kstep=0) -> None:
-    """``b200_sgemm_tf32_ex``: no rounding pass, explicit tuning/debug knobs."""
-    M, N, K = _check_all(a, b, c)
-    _check_device(a, b, c)
-    rc = _capi.lib().b200_sgemm_tf32_ex(
-        a.data_ptr(), b.data_ptr(), c.data_ptr(), M, N, K,
-        _capi.B_ROW_MAJOR_NK if tn else _capi.B_ROW_MAJOR_KN,
-        cta_group, group_m, max_ctas, b_lbo, b_sbo, b_kstep,
-        torch.cuda.current_stream(a.device).cuda_stream)
-    _capi.check(rc, "sgemm_tf32_ex")
 
 
 def tf32_round_(x: torch.Tensor) -> torch.Tensor:

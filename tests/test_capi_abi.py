@@ -16,8 +16,8 @@ def declared_symbols():
 def test_header_declares_expected_entry_points():
     syms = declared_symbols()
     for s in ["b200_version", "b200_last_error", "b200_launch_count", "b200_hgemm_f16",
-              "b200_hgemm_f16_ex", "b200_hgemm_f16_acc16", "b200_hgemm_f16_rows", "b200_hgemm_f16_rows_fused", "b200_fmha_fwd_f16",
-              "b200_hgemm_f16_host", "b200_fmha_fwd_f16_host", "b200_sgemm_tf32", "b200_sgemm_tf32_ex",
+              "b200_hgemm_f16_acc16", "b200_hgemm_f16_rows", "b200_hgemm_f16_rows_fused", "b200_fmha_fwd_f16",
+              "b200_hgemm_f16_host", "b200_fmha_fwd_f16_host", "b200_sgemm_tf32",
               "b200_tf32_round_inplace", "b200_merge_attn_states"]:
         assert s in syms
 
@@ -33,7 +33,7 @@ def test_ctypes_signatures_cover_header(built_lib):
 
 
 def test_version_and_error_text(built_lib):
-    assert built_lib.b200_version() == 1000
+    assert built_lib.b200_version() == 2000
     assert isinstance(built_lib.b200_last_error(), bytes)
 
 

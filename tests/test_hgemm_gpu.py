@@ -28,6 +28,21 @@ def _as_col_major(b):  # reference tools/utils.py:151-156
     return b.t().reshape(b.shape).contiguous()
 
 
+SENT16 = 0x7E5B      # a NaN bit pattern the GEMM never produces
+MARGIN = 256         # elements of C's guard bands (512 B: the alignment of C is kept)
+
+
+def _guarded_c(M, N):
+    """C as a view inside a larger buffer filled with SENT16: (buffer, C)."""
+    buf = torch.empty(M * N + 2 * MARGIN, dtype=torch.half, device="cuda")
+    buf.view(torch.int16).fill_(SENT16)
+    return buf, buf[MARGIN:MARGIN + M * N].view(M, N)
+
+
+def _untouched(t):
+    return bool((t.view(torch.int16) == SENT16).all())
+
+
 def _run(a, b, tn=False, op=None):
     M, K = a.shape
     N = b.shape[1]
@@ -47,13 +62,23 @@ def _run(a, b, tn=False, op=None):
 @pytest.mark.parametrize("tn", [False, True])
 @pytest.mark.parametrize("shape", [(128, 128, 64), (256, 256, 128), (512, 512, 512),
                                    (384, 640, 200), (136, 264, 72), (8, 8, 8), (1000, 24, 4096),
-                                   (128, 24, 512), (128, 64, 512), (1000, 72, 512)])
+                                   (128, 24, 512), (128, 64, 512), (1000, 72, 512), (2600, 2000, 136)])
 def test_vs_oracle_small(shape, tn):
-    """configs[0] (512^3) and ragged shapes the reference cannot run, vs the CPU oracle."""
+    """configs[0] (512^3) and ragged shapes the reference cannot run, vs the CPU oracle, with guard bands around C.
+
+    2600 x 2000 x 136 reaches the partial raster group and the persistent loop: on 132 SMs the host scores 336 tiles of
+    128 x 128 (3 waves, 0.9 x 336 / 396 = 0.76) against 168 of 128 x 256 (2 waves, 168 / 264 = 0.64), so it runs on
+    the 128-column tile, 2-3 tiles per CTA; tiles_m = 21 is a group of 16 m-tiles and then a partial group of 5,
+    which, being odd, walks the n-tiles backwards.  M, N and K are all ragged."""
     M, N, K = shape
     a_np, b_np = hgemm_inputs(M, N, K, seed=M + N + K)
     want = O.hgemm_f32acc(a_np, b_np).astype(np.float32)
-    got = _run(_dev(a_np), _dev(b_np), tn=tn).cpu().numpy().astype(np.float32)
+    a, b = _dev(a_np), _dev(b_np)
+    buf, c = _guarded_c(M, N)
+    hgemm.hgemm(a, _as_col_major(b) if tn else b, c, tn=tn)
+    torch.cuda.synchronize()
+    assert _untouched(buf[:MARGIN]) and _untouched(buf[-MARGIN:]), "store outside C"
+    got = c.cpu().numpy().astype(np.float32)
     np.testing.assert_allclose(got, want, rtol=RTOL, atol=ATOL)
     # and tighter than the tolerance requires: fp32 accumulation differs from the oracle only by
     # summation order, so at most one fp16 ulp of the result
@@ -228,12 +253,14 @@ def test_tile_widths_agree():
     a, b = _dev(a_np), _dev(b_np)
     full = _run(a, b)
     row0, rows = 1024, 256
-    c = torch.full((M, N), float("nan"), dtype=torch.half, device="cuda")
+    buf, c = _guarded_c(M, N)
     rc = _capi.lib().b200_hgemm_f16_rows(a[row0:row0 + rows].data_ptr(), b.data_ptr(), c.data_ptr(), rows, N, K,
                                          _capi.B_ROW_MAJOR_KN, row0, torch.cuda.current_stream().cuda_stream)
     assert rc == 0, _capi.last_error()
     torch.cuda.synchronize()
     assert torch.equal(c[row0:row0 + rows], full[row0:row0 + rows])
+    # the shard call writes its own rows of C and nothing else
+    assert _untouched(buf[:MARGIN + row0 * N]) and _untouched(buf[MARGIN + (row0 + rows) * N:])
 
 
 def test_row_shard_entry_point_matches_full():

@@ -209,8 +209,10 @@ void oracle_attn_online(const uint16_t* q, const uint16_t* k, const uint16_t* v,
 static inline float tf32_of(float x, int mode) {
   uint32_t u;
   memcpy(&u, &x, 4);
-  if ((u & 0x7f800000u) == 0x7f800000u) return x; /* inf / nan unchanged */
-  if (mode == 0) u += 0x1000u;                     /* rna: add half an ulp of the 13 dropped bits */
+  /* rna: add half an ulp of the 13 dropped bits.  Inf and NaN are truncated, not rounded, as cvt.rna.tf32.f32 does
+   * on sm_90: a NaN loses the low 13 bits of its payload (and becomes inf if its payload lay only there).  Mode 1
+   * (truncation) masks NaN payloads the same way. */
+  if (mode == 0 && (u & 0x7f800000u) != 0x7f800000u) u += 0x1000u;
   u &= 0xffffe000u;
   memcpy(&x, &u, 4);
   return x;

@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+import gemm_ref
 from leetcuda_b200 import _capi, hgemm
 from oracle import oracle as O
 from oracle.gen_golden import HGEMM_CASES, hgemm_inputs
@@ -85,6 +86,9 @@ def test_vs_oracle_small(shape, tn):
     truth = O.hgemm_f64(a_np, b_np)
     ulp = np.maximum(np.abs(truth), 1.0) * 2.0 ** -10
     assert np.all(np.abs(got - truth) <= 1.01 * ulp)
+    # and element by element within the bound derived in gemm_ref.py
+    ref = gemm_ref.reference(a_np, b_np, "f16")
+    assert np.all(np.abs(got - ref["c"]) <= gemm_ref.bound(ref))
 
 
 def test_every_op_name_computes_the_same_gemm():

@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 import torch
 
+import gemm_ref
 from leetcuda_b200 import _capi, sgemm
 from oracle import oracle as O
 from oracle.gen_golden import SGEMM_CASES, sgemm_inputs
@@ -52,6 +53,8 @@ def test_vs_oracle_small(shape, tn):
     got = c.cpu().numpy().astype(np.float64)
     assert np.abs(got - truth).max() <= _bound(K, truth)
     assert np.abs(got - O.sgemm_tf32(a_np, b_np, mode="rna")).max() <= _bound(K, truth)
+    ref = gemm_ref.reference(a_np, b_np, "tf32")      # element by element within the bound derived in gemm_ref.py
+    assert np.all(np.abs(got - ref["c"]) <= gemm_ref.bound(ref))
 
 
 def test_unrounded_operands_are_truncated_by_the_tensor_core():

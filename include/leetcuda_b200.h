@@ -123,6 +123,23 @@ int b200_fmha_fwd_f16(const void* q, const void* k, const void* v, void* o, int 
 int b200_fmha_fwd_f16_lse(const void* q, const void* k, const void* v, void* o, float* lse, int B,
                           int H, int N, int D, int v_transposed, float scale, void* stream);
 
+/* Attention with separate query and key lengths and an optional causal mask: prefill against a KV cache, decoding
+ * (Nq << Nk), cross-attention, and the parts of a split-KV computation that b200_merge_attn_states combines.
+ *
+ * q, o: [B,H,Nq,D] contiguous.  k: [B,H,Nk,D].  v: [B,H,Nk,D] (v_transposed = 0) or [B,H,D,Nk] (v_transposed = 1).
+ * lse: [B,H,Nq] fp32, ln sum_j exp(scale * q_i . k_j) over the visible keys, or NULL.  scale <= 0 selects 1/sqrt(D).
+ * causal = 1 masks key j for query i when j > i + (Nk - Nq): the diagonal is aligned bottom-right, as in
+ * FlashAttention-2, so the Nq queries are the last Nq positions of a sequence whose first Nk - Nq keys come from a
+ * cache; with Nq = Nk it is the usual lower triangle.  This is NOT torch SDPA's is_causal when Nq != Nk: SDPA aligns
+ * the diagonal top-left (key j masked when j > i).  With Nq > Nk the rows i < Nq - Nk see no key; such an empty row
+ * gets O = 0 and lse = -inf (never NaN), which b200_merge_attn_states treats as a part without keys.
+ * causal = 0 with Nq = Nk computes exactly what b200_fmha_fwd_f16_lse / b200_fmha_fwd_f16 compute.
+ * Constraints: Nq, Nk >= 1; causal is 0 or 1; D % 8 == 0 and D <= 1024; B * H <= 65535; Nk % 8 == 0 for
+ * v_transposed (for D > 128 V is first restored to [B,H,Nk,D] in stream-ordered scratch, as above).  Numerics as for
+ * b200_fmha_fwd_f16.  A causal CTA visits only the key blocks left of its diagonal, about half the work at Nq = Nk. */
+int b200_fmha_fwd_f16_kv(const void* q, const void* k, const void* v, void* o, float* lse /* may be NULL */,
+                         int B, int H, int Nq, int Nk, int D, int v_transposed, int causal, float scale, void* stream);
+
 /* ------------------------------------------------------------------ SGEMM (TF32)
  * C[M,N] (fp32) = A[M,K] (fp32) x B on the tensor cores through wgmma .tf32 with fp32
  * accumulation — the sibling of the HGEMM path (SURVEY §8f-2).  Replaces

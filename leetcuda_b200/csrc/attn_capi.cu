@@ -13,14 +13,14 @@ using b200::host::fail;
 
 template <int kDS, int kBN, int kWG, bool kVT>
 int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const attn::Params& p, int qtiles,
-                int BH, int smem, cudaStream_t stream) {
-  auto kern = attn::attn_fwd_kernel<kDS, kBN, kWG, kVT>;
-  static int attr_smem[64] = {0};
+                int BH, int smem, bool causal, cudaStream_t stream) {
+  auto kern = causal ? attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true> : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, false>;
+  static int attr_smem[2][64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && attr_smem[dev] < smem) {
+  if (dev >= 0 && dev < 64 && attr_smem[causal][dev] < smem) {
     B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_smem[dev] = smem;
+    attr_smem[causal][dev] = smem;
   }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -64,17 +64,19 @@ __global__ void transpose_dn_to_nd_kernel(const __half* __restrict__ in, __half*
 //   128 < D        256-column slabs (S recomputed per slab), 64-key blocks, one consumer warpgroup (64 query rows)
 // The S, P and O fragments of a consumer thread have to fit its registers: ptxas gives a 384-thread CTA
 // 168 per thread, a 256-thread CTA 255 (O of a 256-column slab alone takes 128).
-int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int H, int N,
-                  int D, bool vt, float scale, cudaStream_t stream) {
+int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int H, int Nq,
+                  int Nk, int D, bool vt, bool causal, float scale, cudaStream_t stream) {
   const uint64_t BH = static_cast<uint64_t>(B) * H;
   const int ds = D <= 64 ? 64 : (D <= 128 ? 128 : 256);
   const int bn = ds == 64 ? 128 : 64;
   const int wgs = ds == 256 ? 1 : 2;
   attn::Params p;
-  p.N = N;
+  p.Nq = Nq;
+  p.Nk = Nk;
   p.D = D;
   p.nq = (D + 63) / 64;
-  p.num_kv = (N + bn - 1) / bn;
+  p.num_kv = (Nk + bn - 1) / bn;
+  p.diag = Nk - Nq;
   p.slabs = (D + ds - 1) / ds;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.lse = lse;
@@ -90,44 +92,48 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
   if (p.ring > 16) p.ring = 16;
   if (p.ring < 2) return fail(B200_ENOTSUP, "headdim not support! (D=%d)", D);
   const int smem = attn::smem_bytes(wgs, slot, p.nq, p.ring);
-  const int qtiles = (N + 64 * wgs - 1) / (64 * wgs);
+  const int qtiles = (Nq + 64 * wgs - 1) / (64 * wgs);
 
   CUtensorMap tq, tk, tv;
-  uint64_t dims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(N), BH};
-  uint64_t str[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(N) * D * 2};
+  uint64_t qdims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(Nq), BH};
+  uint64_t qstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(Nq) * D * 2};
+  uint64_t kdims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(Nk), BH};
+  uint64_t kstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(Nk) * D * 2};
   uint32_t qbox[3] = {64, 64, 1};
   uint32_t kbox[3] = {64, static_cast<uint32_t>(bn), 1};
   int rc;
-  if ((rc = host::get_tmap(&tq, q, 3, dims, str, qbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&tk, k, 3, dims, str, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = host::get_tmap(&tq, q, 3, qdims, qstr, qbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = host::get_tmap(&tk, k, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   if (vt) {
-    uint64_t vd[3] = {static_cast<uint64_t>(N), static_cast<uint64_t>(D), BH};
-    uint64_t vs[2] = {static_cast<uint64_t>(N) * 2, static_cast<uint64_t>(N) * D * 2};
+    uint64_t vd[3] = {static_cast<uint64_t>(Nk), static_cast<uint64_t>(D), BH};
+    uint64_t vs[2] = {static_cast<uint64_t>(Nk) * 2, static_cast<uint64_t>(Nk) * D * 2};
     uint32_t vb[3] = {64, static_cast<uint32_t>(ds), 1};
     if ((rc = host::get_tmap(&tv, v, 3, vd, vs, vb, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   } else {
-    if ((rc = host::get_tmap(&tv, v, 3, dims, str, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    if ((rc = host::get_tmap(&tv, v, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   }
   const int bh = static_cast<int>(BH);
-  if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, stream)
-                          : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, stream);
-  if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, stream)
-                           : launch_attn<128, 64, 2, false>(tq, tk, tv, p, qtiles, bh, smem, stream);
+  if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, stream)
+                          : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, stream);
+  if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, stream)
+                           : launch_attn<128, 64, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, stream);
   if (vt) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with D=%d)", D);
-  return launch_attn<256, 64, 1, false>(tq, tk, tv, p, qtiles, bh, smem, stream);
+  return launch_attn<256, 64, 1, false>(tq, tk, tv, p, qtiles, bh, smem, causal, stream);
 }
 
-int fmha_impl(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int N, int D,
-              int v_transposed, float scale, void* stream_, float rms_g = 0.f) {
+// The checks common to every attention entry and the transpose pre-pass.  The entries with one sequence length pass
+// Nq = Nk = N; b200_fmha_fwd_f16_kv checks its own lengths, causal flag and Nk % 8 first, with messages naming them.
+int fmha_impl(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int Nq, int Nk, int D,
+              int v_transposed, bool causal, float scale, void* stream_, float rms_g = 0.f) {
   if (!q || !k || !v || !o) return fail(B200_EINVAL, "fmha: null pointer");
-  if (B <= 0 || H <= 0 || N <= 0 || D <= 0)
-    return fail(B200_EINVAL, "fmha: bad shape B=%d H=%d N=%d D=%d", B, H, N, D);
+  if (B <= 0 || H <= 0 || Nq <= 0 || Nk <= 0 || D <= 0)
+    return fail(B200_EINVAL, "fmha: bad shape B=%d H=%d N=%d D=%d", B, H, Nq, D);
   if (static_cast<long long>(B) * H > 65535)
     return fail(B200_EINVAL, "fmha: B*H = %lld exceeds the grid limit 65535", static_cast<long long>(B) * H);
   if (D % 8 != 0) return fail(B200_ENOTSUP, "headdim not support! (D=%d must be a multiple of 8)", D);
   if (D > 1024) return fail(B200_ENOTSUP, "headdim not support! (D=%d > 1024)", D);
-  if (v_transposed && (N % 8) != 0)
-    return fail(B200_EINVAL, "fmha: N (%d) must be a multiple of 8 for transposed V", N);
+  if (v_transposed && (Nk % 8) != 0)
+    return fail(B200_EINVAL, "fmha: N (%d) must be a multiple of 8 for transposed V", Nk);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
   if (D > 128) {
@@ -136,23 +142,23 @@ int fmha_impl(const void* q, const void* k, const void* v, void* o, float* lse, 
       // scratch, nothing stays pinned between calls, and neither the allocation nor the free
       // synchronises the device (the memory returns to the pool once this stream passes the free)
       void* ws = nullptr;
-      const size_t bytes = static_cast<size_t>(B) * H * N * D * 2;
+      const size_t bytes = static_cast<size_t>(B) * H * Nk * D * 2;
       B200_CUDA_OK(cudaMallocAsync(&ws, bytes, stream));
-      dim3 grid((N + 31) / 32, (D + 31) / 32, B * H), block(32, 8, 1);
+      dim3 grid((Nk + 31) / 32, (D + 31) / 32, B * H), block(32, 8, 1);
       transpose_dn_to_nd_kernel<<<grid, block, 0, stream>>>(static_cast<const __half*>(v),
-                                                            static_cast<__half*>(ws), D, N);
+                                                            static_cast<__half*>(ws), D, Nk);
       cudaError_t le = cudaGetLastError();
       int rc = 0;
       if (le != cudaSuccess) rc = fail(B200_ECUDA, "transpose launch failed: %s", cudaGetErrorString(le));
       else {
         host::count_launch();
-        rc = fmha_dispatch(q, k, ws, o, lse, rms_g, B, H, N, D, false, scale, stream);
+        rc = fmha_dispatch(q, k, ws, o, lse, rms_g, B, H, Nq, Nk, D, false, causal, scale, stream);
       }
       cudaFreeAsync(ws, stream);
       return rc;
     }
   }
-  return fmha_dispatch(q, k, v, o, lse, rms_g, B, H, N, D, v_transposed != 0, scale, stream);
+  return fmha_dispatch(q, k, v, o, lse, rms_g, B, H, Nq, Nk, D, v_transposed != 0, causal, scale, stream);
 }
 
 }  // namespace
@@ -161,18 +167,27 @@ extern "C" {
 
 int b200_fmha_fwd_f16(const void* q, const void* k, const void* v, void* o, int B, int H, int N,
                       int D, int v_transposed, float scale, void* stream) {
-  return fmha_impl(q, k, v, o, nullptr, B, H, N, D, v_transposed, scale, stream);
+  return fmha_impl(q, k, v, o, nullptr, B, H, N, N, D, v_transposed, false, scale, stream);
 }
 
 int b200_fmha_fwd_f16_lse(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H,
                           int N, int D, int v_transposed, float scale, void* stream) {
   if (!lse) return fail(B200_EINVAL, "fmha_lse: null lse pointer");
-  return fmha_impl(q, k, v, o, lse, B, H, N, D, v_transposed, scale, stream);
+  return fmha_impl(q, k, v, o, lse, B, H, N, N, D, v_transposed, false, scale, stream);
+}
+
+int b200_fmha_fwd_f16_kv(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int Nq,
+                         int Nk, int D, int v_transposed, int causal, float scale, void* stream) {
+  if (Nq <= 0 || Nk <= 0) return fail(B200_EINVAL, "fmha_kv: bad lengths Nq=%d Nk=%d (both must be >= 1)", Nq, Nk);
+  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_kv: causal must be 0 or 1, got %d", causal);
+  if (v_transposed && (Nk % 8) != 0)
+    return fail(B200_EINVAL, "fmha_kv: Nk (%d) must be a multiple of 8 for transposed V", Nk);
+  return fmha_impl(q, k, v, o, lse, B, H, Nq, Nk, D, v_transposed, causal == 1, scale, stream);
 }
 
 int b200_fmha_fwd_f16_rmsnorm(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H,
                               int N, int D, int v_transposed, float scale, float rms_g, void* stream) {
-  return fmha_impl(q, k, v, o, lse, B, H, N, D, v_transposed, scale, stream, rms_g > 0.f ? rms_g : 0.f);
+  return fmha_impl(q, k, v, o, lse, B, H, N, N, D, v_transposed, false, scale, stream, rms_g > 0.f ? rms_g : 0.f);
 }
 
 int b200_fmha_fwd_f16_host(const void* q, const void* k, const void* v, void* o, int B, int H,
@@ -211,7 +226,8 @@ int b200_fmha_fwd_f16_host(const void* q, const void* k, const void* v, void* o,
     B200_CUDA_OK(cudaMemcpyAsync(dv + off, static_cast<const char*>(v) + off, len, cudaMemcpyHostToDevice, pipe.in));
     B200_CUDA_OK(cudaEventRecord(pipe.ev[2 * ci], pipe.in));
     B200_CUDA_OK(cudaStreamWaitEvent(stream, pipe.ev[2 * ci], 0));
-    rc = fmha_impl(dq + off, dk + off, dv + off, dout + off, nullptr, 1, nh, N, D, v_transposed, scale, stream);
+    rc = fmha_impl(dq + off, dk + off, dv + off, dout + off, nullptr, 1, nh, N, N, D, v_transposed, false, scale,
+                   stream);
     if (rc) return rc;
     B200_CUDA_OK(cudaEventRecord(pipe.ev[2 * ci + 1], stream));
     B200_CUDA_OK(cudaStreamWaitEvent(pipe.out, pipe.ev[2 * ci + 1], 0));

@@ -16,6 +16,15 @@
 //     polynomial of softmax_math.cuh), P rounded to fp16 and fed
 //     to P V as the register A operand (the accumulator layout of S is the A-fragment layout);
 //   * O = P V: wgmma m64n64k16 per 64-column chunk of the slab.
+//
+// Queries and keys have their own lengths Nq and Nk.  kCausal masks key j for query i when j > i + (Nk - Nq):
+// the diagonal is aligned bottom-right as in FlashAttention-2, so the last Nq positions of a sequence attend to the
+// Nk - Nq keys before them and to themselves.  This is NOT torch SDPA's is_causal when Nq != Nk (SDPA aligns the
+// diagonal top-left).  With Nq > Nk the query rows i < Nq - Nk see no key: O = 0 and lse = -inf there.
+//   * a CTA visits only the key blocks left of the diagonal of its last query row; both consumer warpgroups run all of
+//     them (they share the K/V ring), so warpgroup 0 may see its last block fully masked;
+//   * the per-element mask runs only in the blocks that cross the diagonal of the warpgroup's rows;
+//   * query tiles are issued in reverse within a head, the longest ones first.
 #pragma once
 #include <cuda.h>
 
@@ -25,13 +34,14 @@ namespace b200 {
 namespace attn {
 
 struct Params {
-  int N, D;
-  int num_kv;          // key blocks of kBN keys
+  int Nq, Nk, D;
+  int num_kv;          // key blocks of kBN keys over Nk
+  int diag;            // Nk - Nq: with kCausal, key j is masked for query i when j > i + diag
   int nq;              // 64-column chunks of D (Q and K)
   int ring;            // K/V ring slots
   int slabs;           // column slabs of O per query tile
   float scale_log2;    // softmax scale * log2(e)
-  float* lse;          // [B*H, N] natural-log LSE, or nullptr
+  float* lse;          // [B*H, Nq] natural-log LSE, or nullptr
   float rms_g;         // > 0: RMS-normalise every output row; with several slabs the CTAs of a query tile form
                        // a cluster and add up the row statistics through distributed shared memory
   __half* o_ptr;
@@ -61,8 +71,16 @@ inline int smem_bytes(int kWG, int slot, int nq, int ring) {
   return kWG * nq * 8192 + ring * slot + 8 * (1 + 2 * ring) + kWG * 64 * 4 + 1024;
 }
 
-// kDS: columns of O per CTA (64, 128 or 256); kBN: keys per block; kVT: V is [B,H,D,N].
-template <int kDS, int kBN, int kWG, bool kVT>
+// Key blocks of kbn keys that a causal CTA whose query rows end before `rows_end` visits.  The producer and the
+// consumers must agree on this count: every block the producer loads is released by every consumer warp.
+__device__ __forceinline__ int causal_kv_blocks(const Params& p, int rows_end, int kbn) {
+  const int keys = rows_end + p.diag;   // keys 0 .. keys - 1 are visible to the CTA's last row
+  return keys <= 0 ? 0 : min(p.num_kv, (keys + kbn - 1) / kbn);
+}
+
+// kDS: columns of O per CTA (64, 128 or 256); kBN: keys per block; kVT: V is [B,H,D,N]; kCausal: the causal mask.
+// kCausal is a template parameter so that the unmasked kernels compile to the code they had without the mask.
+template <int kDS, int kBN, int kWG, bool kVT, bool kCausal>
 __global__ void __launch_bounds__(threads<kWG>(), 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const Params p) {
@@ -85,10 +103,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   auto empty = [&](int s) { return bars + 8u * (1 + p.ring + s); };
 
   const int wg = threadIdx.x / 128, tid = threadIdx.x % 128;
-  const int qtile = blockIdx.x / p.slabs, slab = blockIdx.x % p.slabs;
+  // causal: the last query tile of a head has the most key blocks and starts first.  The head stays on grid.y, so the
+  // resident CTAs still cover few heads and their K / V stays in L2.
+  const int qtile = kCausal ? gridDim.x / p.slabs - 1 - blockIdx.x / p.slabs : blockIdx.x / p.slabs;
+  const int slab = blockIdx.x % p.slabs;
   const int bh = blockIdx.y;
   const int q0 = qtile * 64 * kWG;
   const int d0 = slab * kDS;
+  const int nkv = kCausal ? causal_kv_blocks(p, q0 + 64 * kWG, kBN) : p.num_kv;
   // V chunks of this slab per key block
   const int nvc = kVT ? kBN / 64 : min(NDC, (p.D - d0 + 63) / 64);
 
@@ -120,7 +142,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         ++it;
         return s;
       };
-      for (int j = 0; j < p.num_kv; ++j) {
+      for (int j = 0; j < nkv; ++j) {
         for (int c = 0; c < p.nq; ++c) {
           const int s = next(KV_BYTES);
           tma_load_3d(sring + s * SLOT, &tmap_k, full(s), 64 * c, j * kBN, bh, kEvictLast);
@@ -157,7 +179,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   auto release = [&](int i) {
     if (lane == 0) mbar_arrive(empty(i % p.ring));
   };
-  for (int j = 0; j < p.num_kv; ++j) {
+  const int r0 = q0 + 64 * w;   // first query row of this warpgroup
+  for (int j = 0; j < nkv; ++j) {
     // ---- S = Q K^T over the d-chunks
     float s[NS];
     wg_fence();
@@ -182,15 +205,26 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     // ---- online softmax: this thread holds rows (lane/4) and (lane/4 + 8) of its warp's 16 rows,
     // columns 8 jj + 2 (lane % 4) + {0, 1}: s[4 jj + 2 i + e]
     const int kbase = j * kBN + 2 * (lane % 4);
-    if (j * kBN + kBN > p.N) {
+    if (j * kBN + kBN > p.Nk) {
 #pragma unroll
       for (int jj = 0; jj < kBN / 8; ++jj)
 #pragma unroll
         for (int e = 0; e < 2; ++e)
-          if (kbase + 8 * jj + e >= p.N) {
+          if (kbase + 8 * jj + e >= p.Nk) {
             s[4 * jj + e] = -INFINITY;
             s[4 * jj + 2 + e] = -INFINITY;
           }
+    }
+    if (kCausal && j * kBN + kBN - 1 > r0 + p.diag) {   // the block crosses the diagonal of this warpgroup's rows
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int last = r0 + 16 * warp + lane / 4 + 8 * i + p.diag - kbase;   // last visible key, from kbase
+#pragma unroll
+        for (int jj = 0; jj < kBN / 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (8 * jj + e > last) s[4 * jj + 2 * i + e] = -INFINITY;
+      }
     }
     float alpha[2];
 #pragma unroll
@@ -201,14 +235,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       const float mn = fmaxf(m[i], mx * p.scale_log2);
-      alpha[i] = fast_exp2(m[i] - mn);
+      // a row without a visible key so far (causal only): subtract 0, so that alpha and x are exp2(-inf), not NaN
+      const float mb = kCausal && mn == -INFINITY ? 0.f : mn;
+      alpha[i] = fast_exp2(m[i] - mb);
       m[i] = mn;
       float sum = 0.f;
 #pragma unroll
       for (int jj = 0; jj < kBN / 8; ++jj)
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          const float x = fmaf(s[4 * jj + 2 * i + e], p.scale_log2, -mn);
+          const float x = fmaf(s[4 * jj + 2 * i + e], p.scale_log2, -mb);
           const float pe = ((kPolyMask >> (4 * (jj % 4))) & 1u) ? exp2_fma_pipe(x) : fast_exp2(x);
           s[4 * jj + 2 * i + e] = pe;
           sum += pe;
@@ -266,7 +302,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
 
   // ---- epilogue
-  const size_t head = static_cast<size_t>(bh) * p.N;
+  const size_t head = static_cast<size_t>(bh) * p.Nq;
   float inv[2], lsum[2], ss[2];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
@@ -274,7 +310,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     lt += __shfl_xor_sync(0xffffffffu, lt, 1);
     lt += __shfl_xor_sync(0xffffffffu, lt, 2);
     lsum[i] = lt;
-    inv[i] = 1.f / lt;
+    // an empty row is told by m, not by l: exp2_fma_pipe(-inf) = 2^-126 leaves l slightly above 0
+    inv[i] = kCausal && m[i] == -INFINITY ? 0.f : 1.f / lt;
     ss[i] = 0.f;
     if (p.rms_g > 0.f) {
 #pragma unroll
@@ -313,8 +350,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   for (int i = 0; i < 2; ++i) {
     if (p.rms_g > 0.f) inv[i] *= rsqrtf(ss[i] / static_cast<float>(p.D) + 1e-5f) * p.rms_g;
     const int row = q0 + 64 * w + 16 * warp + lane / 4 + 8 * i;
-    if (row >= p.N) continue;
-    if (p.lse && slab == 0 && (lane % 4) == 0) p.lse[head + row] = (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
+    if (row >= p.Nq) continue;
+    if (p.lse && slab == 0 && (lane % 4) == 0)
+      p.lse[head + row] = kCausal && m[i] == -INFINITY ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
     __half* orow = p.o_ptr + (head + row) * p.D;
 #pragma unroll
     for (int c = 0; c < NDC; ++c)

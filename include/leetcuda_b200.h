@@ -140,6 +140,34 @@ int b200_fmha_fwd_f16_lse(const void* q, const void* k, const void* v, void* o, 
 int b200_fmha_fwd_f16_kv(const void* q, const void* k, const void* v, void* o, float* lse /* may be NULL */,
                          int B, int H, int Nq, int Nk, int D, int v_transposed, int causal, float scale, void* stream);
 
+/* Grouped-query attention (GQA / MQA) and split-KV decoding: b200_fmha_fwd_f16_kv with fewer K/V heads than query heads,
+ * and the keys of every CTA optionally cut into num_splits ranges that run in parallel.
+ *
+ * q, o: [B,H,Nq,D] contiguous.  k: [B,Hkv,Nk,D].  v: [B,Hkv,Nk,D] (v_transposed = 0) or [B,Hkv,D,Nk] (v_transposed = 1).
+ * lse: [B,H,Nq] fp32 or NULL.  H % Hkv == 0; query head h reads K/V head h / (H / Hkv), the convention of torch SDPA's
+ * enable_gqa and of FlashAttention.  Hkv == H is multi-head and Hkv == 1 multi-query attention.  Causal masking, empty
+ * rows (O = 0, lse = -inf), scale, lse and numerics are those of b200_fmha_fwd_f16_kv.  The H / Hkv query heads of a
+ * K/V head run as one tile of packed rows, so each K/V block is read once per group and a decode step fills
+ * H / Hkv rows of the tile instead of one.
+ * num_splits = 1: no split, one launch (with transposed V and D > 128 the pre-pass is a second one), and O, lse equal
+ * those of b200_fmha_fwd_f16_kv on K and V with every head repeated H / Hkv times, bit for bit.  num_splits = n > 1:
+ * the key blocks each CTA visits are cut into n contiguous ranges (a range may be empty and then contributes nothing);
+ * every split writes its normalised O in fp32 and its lse to a stream-ordered workspace (cudaMallocAsync /
+ * cudaFreeAsync on `stream`, (n * B * H * Nq * (D + 1)) * 4 bytes), and a second launch combines the parts with their
+ * lse weights and rounds once to fp16.  num_splits = 0 lets the library choose from the shapes and the SM count: 1 when
+ * the unsplit grid already fills the GPU, otherwise enough splits to cover the SMs once — the choice for decoding.
+ * Constraints: those of b200_fmha_fwd_f16_kv, with the grid limit on B * Hkv <= 65535 instead of B * H;
+ * Hkv >= 1 and H % Hkv == 0; 0 <= num_splits <= B200_FMHA_MAX_SPLITS; with num_splits != 1, o 16-byte aligned (the
+ * combine stores 16-byte packs; a tensor from a CUDA allocator is). */
+#define B200_FMHA_MAX_SPLITS 64
+int b200_fmha_fwd_f16_gqa(const void* q, const void* k, const void* v, void* o, float* lse /* may be NULL */,
+                          int B, int H, int Hkv, int Nq, int Nk, int D, int v_transposed, int causal,
+                          int num_splits, float scale, void* stream);
+
+/* The split count b200_fmha_fwd_f16_gqa chooses for num_splits = 0 on the current device (>= 1), or a negative
+ * B200_E* code for a bad shape.  Depends on the shapes and the device's SM count only (not on causal or the layout). */
+int b200_fmha_fwd_f16_gqa_splits(int B, int H, int Hkv, int Nq, int Nk, int D);
+
 /* ------------------------------------------------------------------ SGEMM (TF32)
  * C[M,N] (fp32) = A[M,K] (fp32) x B on the tensor cores through wgmma .tf32 with fp32
  * accumulation — the sibling of the HGEMM path (SURVEY §8f-2).  Replaces

@@ -19,6 +19,7 @@ LIB_PATH = _HERE / "libleetcuda_b200.so"
 B200_OK = 0
 B_ROW_MAJOR_KN = 0  # "NN"
 B_ROW_MAJOR_NK = 1  # "TN"
+FMHA_MAX_SPLITS = 64  # B200_FMHA_MAX_SPLITS
 
 _lib = None
 
@@ -38,6 +39,8 @@ SIGNATURES = {
     "b200_fmha_fwd_f16": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
     "b200_fmha_fwd_f16_lse": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
     "b200_fmha_fwd_f16_kv": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _vp]),
+    "b200_fmha_fwd_f16_gqa": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _vp]),
+    "b200_fmha_fwd_f16_gqa_splits": (_i, [_i, _i, _i, _i, _i, _i]),
     "b200_fmha_fwd_f16_rmsnorm": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
     "b200_rope_f32": (_i, [_vp, _vp, _i, _i, _vp]),
     "b200_rope_qk_f16": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),

@@ -1,7 +1,10 @@
 // attn_capi.cu — C-ABI entry points of the attention path (include/leetcuda_b200.h).
 #include <math.h>
+#include <float.h>
 #include <stdlib.h>
 #include <string.h>
+
+#include <algorithm>
 
 #include "capi_common.cuh"
 #include "attn_sm90.cuh"
@@ -11,20 +14,36 @@ namespace {
 using namespace b200;
 using b200::host::fail;
 
+// Split-KV: the most splits b200_fmha_fwd_f16_gqa accepts (B200_FMHA_MAX_SPLITS); for num_splits = 0 the fewest key
+// blocks a split keeps, and the fewest key blocks of a CTA worth splitting at all.  Measured on an H100 80GB HBM3
+// (400 W, 1980 MHz), D = 128, one CTA (B1 H8 Hkv1 and B1 H32 Hkv4, Nq = 1), fixed split counts timed alternately:
+// at 8 key blocks (Nk = 512) every split was slower than none (0.024 ms unsplit, >= 0.029 ms split: the combine launch
+// and the workspace cost more than they save); from 16 blocks on, splits of about 4 blocks were as fast as the best
+// count or within its spread (Nk = 2048: 8 splits 0.039 .. 0.046 ms, 4 splits 0.046, unsplit 0.072 ms).
+constexpr int kMaxSplits = 64;
+constexpr int kMinBlocksPerSplit = 4;
+constexpr int kMinBlocksToSplit = 16;
+
 template <int kDS, int kBN, int kWG, bool kVT>
 int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const attn::Params& p, int qtiles,
-                int BH, int smem, bool causal, cudaStream_t stream) {
-  auto kern = causal ? attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true> : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, false>;
-  static int attr_smem[2][64] = {};
+                int BH, int smem, bool causal, bool packed, int splits, cudaStream_t stream) {
+  // packed query heads need the kGQA kernels only for the mask; a split always runs a kSplit kernel
+  auto kern = splits > 1 ? (causal ? attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true, true, true>
+                                   : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, false, false, true>)
+                         : (causal ? (packed ? attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true, true>
+                                             : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true>)
+                                   : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, false>);
+  const int variant = splits > 1 ? 3 + causal : causal + (causal && packed);
+  static int attr_smem[5][64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && attr_smem[causal][dev] < smem) {
+  if (dev >= 0 && dev < 64 && attr_smem[variant][dev] < smem) {
     B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_smem[causal][dev] = smem;
+    attr_smem[variant][dev] = smem;
   }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(static_cast<unsigned>(qtiles * p.slabs), static_cast<unsigned>(BH), 1);
+  cfg.gridDim = dim3(static_cast<unsigned>(qtiles * p.slabs), static_cast<unsigned>(BH), static_cast<unsigned>(splits));
   cfg.blockDim = dim3(attn::threads<kWG>(), 1, 1);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
@@ -58,20 +77,86 @@ __global__ void transpose_dn_to_nd_kernel(const __half* __restrict__ in, __half*
   }
 }
 
+// out[r, :] = sum_s w_s o_s[r, :] / sum_s w_s,  w_s = exp(lse_s[r] - max_s lse_s[r]),  out_lse[r] = ln sum_s w_s + max
+// over the fp32 parts the split kernel wrote (ws_o [splits, rows, D], ws_lse [splits, rows]), rounded once to fp16.  A
+// row whose parts are all empty (lse -inf) gets 0 and -inf: the max is clamped to -FLT_MAX, every weight is 0, and the
+// divisor is clamped to 1 (otherwise one weight is expf(0) = 1, so the clamp changes nothing).
+// HBM-bound: one thread per 16-byte pack of the output (8 halves), 32 bytes and one lse read per split.
+template <typename Idx>
+__global__ void __launch_bounds__(256)
+attn_combine_kernel(__half* __restrict__ out, float* __restrict__ out_lse, const float* __restrict__ ws_o,
+                    const float* __restrict__ ws_lse, unsigned rows, unsigned packs_per_row, int splits) {
+  const Idx n_packs = static_cast<Idx>(rows) * packs_per_row;
+  const Idx pk = static_cast<Idx>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (pk >= n_packs) return;
+  const Idx row = pk / packs_per_row;
+  const size_t part = static_cast<size_t>(n_packs) * 8;   // floats of one split's O
+  const float* src = ws_o + static_cast<size_t>(pk) * 8;
+  float top = -FLT_MAX;
+  for (int s = 0; s < splits; ++s) top = fmaxf(top, __ldg(ws_lse + static_cast<size_t>(s) * rows + row));
+  float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  float denom = 0.f;
+  for (int s = 0; s < splits; ++s) {
+    const uint4 a = ld_stream(src + s * part), b = ld_stream(src + s * part + 4);
+    const float w = expf(__ldg(ws_lse + static_cast<size_t>(s) * rows + row) - top);
+    const float x[8] = {__uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z), __uint_as_float(a.w),
+                        __uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z), __uint_as_float(b.w)};
+    denom += w;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] = fmaf(w, x[e], acc[e]);
+  }
+  const float inv = 1.f / fmaxf(denom, 1.f);
+  uint4 r;
+  r.x = pack_half2(acc[0] * inv, acc[1] * inv);
+  r.y = pack_half2(acc[2] * inv, acc[3] * inv);
+  r.z = pack_half2(acc[4] * inv, acc[5] * inv);
+  r.w = pack_half2(acc[6] * inv, acc[7] * inv);
+  st_stream(reinterpret_cast<uint4*>(out) + pk, r);
+  if (out_lse != nullptr && pk == row * packs_per_row) out_lse[row] = logf(denom) + top;   // first pack of the row
+}
+
+int launch_combine(__half* out, float* out_lse, const float* ws_o, const float* ws_lse, size_t rows, int D, int splits,
+                   cudaStream_t stream) {
+  const unsigned ppr = static_cast<unsigned>(D / 8);
+  const size_t total = rows * ppr;
+  const size_t blocks = (total + 255) / 256;
+  if (rows > 0xFFFFFFFFull || blocks > 0x7FFFFFFFull) return fail(B200_EINVAL, "fmha_gqa: too many output rows");
+  const unsigned g = static_cast<unsigned>(blocks), nr = static_cast<unsigned>(rows);
+  if (total + 256 < 0xFFFFFFFFull)
+    attn_combine_kernel<unsigned><<<g, 256, 0, stream>>>(out, out_lse, ws_o, ws_lse, nr, ppr, splits);
+  else
+    attn_combine_kernel<size_t><<<g, 256, 0, stream>>>(out, out_lse, ws_o, ws_lse, nr, ppr, splits);
+  B200_CUDA_OK(cudaGetLastError());
+  host::count_launch();
+  return 0;
+}
+
 // Kernel shape per head dim (attn_sm90.cuh):
 //   D <= 64        one 64-column slab, 128-key blocks, two consumer warpgroups (128 query rows)
 //   64 < D <= 128  one 128-column slab, 64-key blocks, two consumer warpgroups
 //   128 < D        256-column slabs (S recomputed per slab), 64-key blocks, one consumer warpgroup (64 query rows)
 // The S, P and O fragments of a consumer thread have to fit its registers: ptxas gives a 384-thread CTA
 // 168 per thread, a 256-thread CTA 255 (O of a 256-column slab alone takes 128).
-int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int H, int Nq,
-                  int Nk, int D, bool vt, bool causal, float scale, cudaStream_t stream) {
-  const uint64_t BH = static_cast<uint64_t>(B) * H;
+struct Family {
+  int ds, bn, wgs;
+};
+Family family(int D) {
   const int ds = D <= 64 ? 64 : (D <= 128 ? 128 : 256);
-  const int bn = ds == 64 ? 128 : 64;
-  const int wgs = ds == 256 ? 1 : 2;
+  return {ds, ds == 64 ? 128 : 64, ds == 256 ? 1 : 2};
+}
+
+// G: query heads per K/V head (H = G * Hkv; the kernel sees B * Hkv heads of G * Nq packed rows).  splits > 1: grid.z
+// splits whose fp32 parts go to ws_o / ws_lse instead of o / lse (kSplit kernels).  Causal with G > 1 runs kGQA.
+int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int Hkv, int G,
+                  int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, float* ws_o, float* ws_lse,
+                  cudaStream_t stream) {
+  const uint64_t BH = static_cast<uint64_t>(B) * Hkv;
+  const Family f = family(D);
+  const int ds = f.ds, bn = f.bn, wgs = f.wgs;
+  const int rows = G * Nq;   // packed rows per K/V head
   attn::Params p;
-  p.Nq = Nq;
+  p.Nq = rows;
+  p.qpos = Nq;
   p.Nk = Nk;
   p.D = D;
   p.nq = (D + 63) / 64;
@@ -82,6 +167,8 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
   p.lse = lse;
   p.rms_g = rms_g;
   p.o_ptr = static_cast<__half*>(o);
+  p.ws_o = splits > 1 ? ws_o : nullptr;
+  p.ws_lse = splits > 1 ? ws_lse : nullptr;
   if (rms_g > 0.f && D > 256 && !(D <= 512 && D % 128 == 0))
     return fail(B200_ENOTSUP, "fused rms_norm: D=%d (supported: D <= 256, 384, 512)", D);
   // ring: every slot that fits next to Q, at most 16 (two key blocks of K and V chunks at D = 512)
@@ -92,11 +179,13 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
   if (p.ring > 16) p.ring = 16;
   if (p.ring < 2) return fail(B200_ENOTSUP, "headdim not support! (D=%d)", D);
   const int smem = attn::smem_bytes(wgs, slot, p.nq, p.ring);
-  const int qtiles = (Nq + 64 * wgs - 1) / (64 * wgs);
+  // causal packed heads of at least one tile of rows: tiles of their own per head (attn_sm90.cuh), else packed tiles
+  p.tph = causal && Nq >= 64 * wgs ? (Nq + 64 * wgs - 1) / (64 * wgs) : 0;
+  const int qtiles = p.tph > 0 ? G * p.tph : (rows + 64 * wgs - 1) / (64 * wgs);
 
   CUtensorMap tq, tk, tv;
-  uint64_t qdims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(Nq), BH};
-  uint64_t qstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(Nq) * D * 2};
+  uint64_t qdims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(rows), BH};
+  uint64_t qstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(rows) * D * 2};
   uint64_t kdims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(Nk), BH};
   uint64_t kstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(Nk) * D * 2};
   uint32_t qbox[3] = {64, 64, 1};
@@ -113,38 +202,83 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
     if ((rc = host::get_tmap(&tv, v, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   }
   const int bh = static_cast<int>(BH);
-  if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, stream)
-                          : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, stream);
-  if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, stream)
-                           : launch_attn<128, 64, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, stream);
+  if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, G > 1, splits, stream)
+                          : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, G > 1, splits, stream);
+  if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, G > 1, splits, stream)
+                           : launch_attn<128, 64, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, G > 1, splits, stream);
   if (vt) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with D=%d)", D);
-  return launch_attn<256, 64, 1, false>(tq, tk, tv, p, qtiles, bh, smem, causal, stream);
+  return launch_attn<256, 64, 1, false>(tq, tk, tv, p, qtiles, bh, smem, causal, G > 1, splits, stream);
+}
+
+// The attention kernel, and with splits > 1 its fp32 parts in a stream-ordered workspace and the combine kernel.
+int fmha_run(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int Hkv, int G,
+             int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, cudaStream_t stream) {
+  if (splits <= 1)
+    return fmha_dispatch(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, 1, nullptr, nullptr, stream);
+  const size_t rows = static_cast<size_t>(B) * Hkv * G * Nq;
+  const size_t lse_bytes = (static_cast<size_t>(splits) * rows * 4 + 255) & ~static_cast<size_t>(255);
+  void* ws = nullptr;
+  B200_CUDA_OK(cudaMallocAsync(&ws, lse_bytes + static_cast<size_t>(splits) * rows * D * 4, stream));
+  float* ws_lse = static_cast<float*>(ws);
+  float* ws_o = reinterpret_cast<float*>(static_cast<char*>(ws) + lse_bytes);
+  int rc = fmha_dispatch(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, splits, ws_o, ws_lse, stream);
+  if (rc == 0) rc = launch_combine(static_cast<__half*>(o), lse, ws_o, ws_lse, rows, D, splits, stream);
+  cudaFreeAsync(ws, stream);
+  return rc;
+}
+
+// num_splits = 0: split until the grid covers the SMs once (a CTA takes a whole SM, so a second wave of shorter CTAs
+// would not finish sooner), keeping at least kMinBlocksPerSplit key blocks per split; 1 when the grid already fills
+// the machine or the keys span fewer than kMinBlocksToSplit blocks.
+int auto_splits(int B, int Hkv, int G, int Nq, int Nk, int D) {
+  static int sms[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  int n = dev >= 0 && dev < 64 ? sms[dev] : 0;
+  if (n == 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 1;
+    if (dev >= 0 && dev < 64) sms[dev] = n;
+  }
+  const Family f = family(D);
+  const long long rows = static_cast<long long>(G) * Nq;
+  const long long ctas = (rows + 64 * f.wgs - 1) / (64 * f.wgs) * ((D + f.ds - 1) / f.ds) * B * Hkv;
+  const long long num_kv = (Nk + f.bn - 1) / f.bn;
+  if (ctas >= n || num_kv < kMinBlocksToSplit) return 1;
+  long long s = n / ctas;
+  s = std::min<long long>(s, num_kv / kMinBlocksPerSplit);
+  s = std::min<long long>(s, kMaxSplits);
+  return s < 1 ? 1 : static_cast<int>(s);
 }
 
 // The checks common to every attention entry and the transpose pre-pass.  The entries with one sequence length pass
-// Nq = Nk = N; b200_fmha_fwd_f16_kv checks its own lengths, causal flag and Nk % 8 first, with messages naming them.
+// Nq = Nk = N; b200_fmha_fwd_f16_kv checks its own lengths, causal flag and Nk % 8 first, with messages naming them;
+// b200_fmha_fwd_f16_gqa also its head counts and splits.  G: query heads per K/V head (K and V have H / G heads);
+// splits = 0 picks the split count (auto_splits).
 int fmha_impl(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int Nq, int Nk, int D,
-              int v_transposed, bool causal, float scale, void* stream_, float rms_g = 0.f) {
+              int v_transposed, bool causal, float scale, void* stream_, float rms_g = 0.f, int G = 1,
+              int splits = 1) {
   if (!q || !k || !v || !o) return fail(B200_EINVAL, "fmha: null pointer");
   if (B <= 0 || H <= 0 || Nq <= 0 || Nk <= 0 || D <= 0)
     return fail(B200_EINVAL, "fmha: bad shape B=%d H=%d N=%d D=%d", B, H, Nq, D);
-  if (static_cast<long long>(B) * H > 65535)
-    return fail(B200_EINVAL, "fmha: B*H = %lld exceeds the grid limit 65535", static_cast<long long>(B) * H);
+  const int Hkv = H / G;
+  if (static_cast<long long>(B) * Hkv > 65535)
+    return fail(B200_EINVAL, "fmha: B*H = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
   if (D % 8 != 0) return fail(B200_ENOTSUP, "headdim not support! (D=%d must be a multiple of 8)", D);
   if (D > 1024) return fail(B200_ENOTSUP, "headdim not support! (D=%d > 1024)", D);
   if (v_transposed && (Nk % 8) != 0)
     return fail(B200_EINVAL, "fmha: N (%d) must be a multiple of 8 for transposed V", Nk);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
+  if (splits == 0) splits = auto_splits(B, Hkv, G, Nq, Nk, D);
   if (D > 128) {
     if (v_transposed) {
       // the restored V lives in a stream-ordered allocation: calls on different streams never share
       // scratch, nothing stays pinned between calls, and neither the allocation nor the free
       // synchronises the device (the memory returns to the pool once this stream passes the free)
       void* ws = nullptr;
-      const size_t bytes = static_cast<size_t>(B) * H * Nk * D * 2;
+      const size_t bytes = static_cast<size_t>(B) * Hkv * Nk * D * 2;
       B200_CUDA_OK(cudaMallocAsync(&ws, bytes, stream));
-      dim3 grid((Nk + 31) / 32, (D + 31) / 32, B * H), block(32, 8, 1);
+      dim3 grid((Nk + 31) / 32, (D + 31) / 32, B * Hkv), block(32, 8, 1);
       transpose_dn_to_nd_kernel<<<grid, block, 0, stream>>>(static_cast<const __half*>(v),
                                                             static_cast<__half*>(ws), D, Nk);
       cudaError_t le = cudaGetLastError();
@@ -152,13 +286,13 @@ int fmha_impl(const void* q, const void* k, const void* v, void* o, float* lse, 
       if (le != cudaSuccess) rc = fail(B200_ECUDA, "transpose launch failed: %s", cudaGetErrorString(le));
       else {
         host::count_launch();
-        rc = fmha_dispatch(q, k, ws, o, lse, rms_g, B, H, Nq, Nk, D, false, causal, scale, stream);
+        rc = fmha_run(q, k, ws, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, false, causal, scale, splits, stream);
       }
       cudaFreeAsync(ws, stream);
       return rc;
     }
   }
-  return fmha_dispatch(q, k, v, o, lse, rms_g, B, H, Nq, Nk, D, v_transposed != 0, causal, scale, stream);
+  return fmha_run(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, v_transposed != 0, causal, scale, splits, stream);
 }
 
 }  // namespace
@@ -183,6 +317,36 @@ int b200_fmha_fwd_f16_kv(const void* q, const void* k, const void* v, void* o, f
   if (v_transposed && (Nk % 8) != 0)
     return fail(B200_EINVAL, "fmha_kv: Nk (%d) must be a multiple of 8 for transposed V", Nk);
   return fmha_impl(q, k, v, o, lse, B, H, Nq, Nk, D, v_transposed, causal == 1, scale, stream);
+}
+
+int b200_fmha_fwd_f16_gqa(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int Hkv,
+                          int Nq, int Nk, int D, int v_transposed, int causal, int num_splits, float scale,
+                          void* stream) {
+  if (Nq <= 0 || Nk <= 0) return fail(B200_EINVAL, "fmha_gqa: bad lengths Nq=%d Nk=%d (both must be >= 1)", Nq, Nk);
+  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_gqa: causal must be 0 or 1, got %d", causal);
+  if (v_transposed && (Nk % 8) != 0)
+    return fail(B200_EINVAL, "fmha_gqa: Nk (%d) must be a multiple of 8 for transposed V", Nk);
+  if (Hkv <= 0 || H % Hkv != 0)
+    return fail(B200_EINVAL, "fmha_gqa: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
+  if (num_splits < 0 || num_splits > kMaxSplits)
+    return fail(B200_EINVAL, "fmha_gqa: num_splits=%d must be in 0 .. %d", num_splits, kMaxSplits);
+  if (static_cast<long long>(B) * Hkv > 65535)
+    return fail(B200_EINVAL, "fmha_gqa: B*Hkv = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
+  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
+    return fail(B200_EINVAL, "fmha_gqa: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)");
+  if (static_cast<long long>(H / Hkv) * Nq > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "fmha_gqa: (H/Hkv)*Nq = %lld query rows per K/V head exceed 2^31 - 1",
+                static_cast<long long>(H / Hkv) * Nq);
+  return fmha_impl(q, k, v, o, lse, B, H, Nq, Nk, D, v_transposed, causal == 1, scale, stream, 0.f, H / Hkv,
+                   num_splits);
+}
+
+int b200_fmha_fwd_f16_gqa_splits(int B, int H, int Hkv, int Nq, int Nk, int D) {
+  if (B <= 0 || H <= 0 || Nq <= 0 || Nk <= 0 || D <= 0)
+    return fail(B200_EINVAL, "fmha_gqa_splits: bad shape B=%d H=%d Nq=%d Nk=%d D=%d", B, H, Nq, Nk, D);
+  if (Hkv <= 0 || H % Hkv != 0)
+    return fail(B200_EINVAL, "fmha_gqa_splits: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
+  return auto_splits(B, Hkv, H / Hkv, Nq, Nk, D);
 }
 
 int b200_fmha_fwd_f16_rmsnorm(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H,

@@ -25,6 +25,17 @@
 //     them (they share the K/V ring), so warpgroup 0 may see its last block fully masked;
 //   * the per-element mask runs only in the blocks that cross the diagonal of the warpgroup's rows;
 //   * query tiles are issued in reverse within a head, the longest ones first.
+//
+// Grouped-query attention and split-KV (b200_fmha_fwd_f16_gqa):
+//   * Packing: query head h reads K/V head h / G.  The G query heads of one KV group are contiguous in Q [B,H,Nq,D],
+//     so they form one [G*Nq, D] "head" of packed rows and grid.y walks the B*Hkv KV heads.  Without the mask that
+//     is the plain kernel with G*Nq rows; with it (kGQA) packed row r has the query position r % Nq, which the
+//     causal mask, the diagonal test and the block count use.  With Nq >= the tile rows, each query head gets tiles of
+//     its own (tph per head, longest first across the G heads): the tiles and the work are those of the expanded
+//     kernel and positions are row - g * Nq.  Shorter heads (decoding) are packed across head boundaries, so a tile
+//     holds the rows of several heads.
+//   * kSplit: grid.z cuts the key blocks [0, nkv) a CTA visits into contiguous ranges; the epilogue writes the
+//     split's normalised O in fp32 and its lse to a workspace that a combine kernel reduces.
 #pragma once
 #include <cuda.h>
 
@@ -34,7 +45,7 @@ namespace b200 {
 namespace attn {
 
 struct Params {
-  int Nq, Nk, D;
+  int Nq, Nk, D;       // Nq: rows of a head (kGQA: G * Nq packed rows of one KV group)
   int num_kv;          // key blocks of kBN keys over Nk
   int diag;            // Nk - Nq: with kCausal, key j is masked for query i when j > i + diag
   int nq;              // 64-column chunks of D (Q and K)
@@ -45,6 +56,11 @@ struct Params {
   float rms_g;         // > 0: RMS-normalise every output row; with several slabs the CTAs of a query tile form
                        // a cluster and add up the row statistics through distributed shared memory
   __half* o_ptr;
+  float* ws_o;         // kSplit: [splits, B*H*Nq', D] fp32 normalised O of every split
+  float* ws_lse;       //                          [splits, B*H*Nq'] natural-log LSE of every split
+  int qpos;            // kGQA: query positions per head (the call's Nq); packed row r has position r % qpos
+  int tph;             // kGQA: > 0: every query head has its own tph tiles (no tile straddles two heads), 0: the
+                       // tiles cut the packed rows of the group
 };
 
 // Keys whose exponential the D <= 128 kernels evaluate on the FMA pipe (exp2_fma_pipe) instead of MUFU.EX2: bit i
@@ -78,9 +94,37 @@ __device__ __forceinline__ int causal_kv_blocks(const Params& p, int rows_end, i
   return keys <= 0 ? 0 : min(p.num_kv, (keys + kbn - 1) / kbn);
 }
 
-// kDS: columns of O per CTA (64, 128 or 256); kBN: keys per block; kVT: V is [B,H,D,N]; kCausal: the causal mask.
-// kCausal is a template parameter so that the unmasked kernels compile to the code they had without the mask.
-template <int kDS, int kBN, int kWG, bool kVT, bool kCausal>
+// The key blocks [x, y) of a CTA whose rows start at q0: with kCausal the blocks left of the diagonal of its greatest
+// query position (kGQA: of a packed row), with kSplit the grid.z-th of gridDim.z contiguous ranges of them (possibly
+// empty).  The producer and the consumers both take their loop bounds from here.
+// kGQA: the CTA's rows [q0, row_end) are query positions from q0 - off on (per-head tiles), or packed rows (p.tph = 0).
+template <int kBN, int kRows, bool kCausal, bool kGQA, bool kSplit>
+__device__ __forceinline__ int2 kv_blocks(const Params& p, int q0, int row_end, int off) {
+  int nkv = p.num_kv;
+  if constexpr (kCausal) {
+    int rows_end = q0 + kRows;
+    if constexpr (kGQA) {
+      if (p.tph > 0) {
+        rows_end = min(rows_end, row_end) - off;
+      } else {
+        // packed rows: a tile that crosses into the next query head (or ends the group) holds position Nq - 1
+        const int last = min(rows_end, p.Nq) - 1;
+        rows_end = last / p.qpos != q0 / p.qpos ? p.qpos : last % p.qpos + 1;
+      }
+    }
+    nkv = causal_kv_blocks(p, rows_end, kBN);
+  }
+  if constexpr (kSplit) {
+    const long long z = blockIdx.z, splits = gridDim.z;
+    return make_int2(static_cast<int>(nkv * z / splits), static_cast<int>(nkv * (z + 1) / splits));
+  }
+  return make_int2(0, nkv);
+}
+
+// kDS: columns of O per CTA (64, 128 or 256); kBN: keys per block; kVT: V is [B,H,D,N]; kCausal: the causal mask;
+// kGQA: the causal mask on packed query heads; kSplit: split-KV (see the top of this file).
+// kCausal, kGQA and kSplit are template parameters so that the other kernels compile to the code they had without them.
+template <int kDS, int kBN, int kWG, bool kVT, bool kCausal, bool kGQA = false, bool kSplit = false>
 __global__ void __launch_bounds__(threads<kWG>(), 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const Params p) {
@@ -106,11 +150,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   // causal: the last query tile of a head has the most key blocks and starts first.  The head stays on grid.y, so the
   // resident CTAs still cover few heads and their K / V stays in L2.
   const int qtile = kCausal ? gridDim.x / p.slabs - 1 - blockIdx.x / p.slabs : blockIdx.x / p.slabs;
+  int q0 = qtile * 64 * kWG;
+  int row_end = p.Nq, off = 0;   // kGQA: the rows this CTA stores end before row_end; query position = row - off
+  if constexpr (kCausal && kGQA) {
+    if (p.tph > 0) {
+      // per-head tiles, the longest first across the G heads of the group, not only within one
+      const int x = blockIdx.x / p.slabs, G = gridDim.x / p.slabs / p.tph;
+      off = (x % G) * p.qpos;
+      q0 = off + (p.tph - 1 - x / G) * 64 * kWG;
+      row_end = off + p.qpos;
+    }
+  }
   const int slab = blockIdx.x % p.slabs;
   const int bh = blockIdx.y;
-  const int q0 = qtile * 64 * kWG;
   const int d0 = slab * kDS;
-  const int nkv = kCausal ? causal_kv_blocks(p, q0 + 64 * kWG, kBN) : p.num_kv;
+  const int2 kv = kv_blocks<kBN, 64 * kWG, kCausal, kGQA, kSplit>(p, q0, row_end, off);
   // V chunks of this slab per key block
   const int nvc = kVT ? kBN / 64 : min(NDC, (p.D - d0 + 63) / 64);
 
@@ -142,7 +196,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         ++it;
         return s;
       };
-      for (int j = 0; j < nkv; ++j) {
+      for (int j = kv.x; j < kv.y; ++j) {
         for (int c = 0; c < p.nq; ++c) {
           const int s = next(KV_BYTES);
           tma_load_3d(sring + s * SLOT, &tmap_k, full(s), 64 * c, j * kBN, bh, kEvictLast);
@@ -180,7 +234,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     if (lane == 0) mbar_arrive(empty(i % p.ring));
   };
   const int r0 = q0 + 64 * w;   // first query row of this warpgroup
-  for (int j = 0; j < nkv; ++j) {
+  // kGQA: query positions of packed rows for the mask: the least one of the warpgroup's rows, and those of this
+  // thread's two rows (without kGQA a row's position is the row)
+  int pos0 = 0, pos[2] = {0, 0};
+  if constexpr (kCausal && kGQA) {
+    if (p.tph > 0) {
+      pos0 = r0 - off;
+      pos[0] = r0 + 16 * warp + lane / 4 - off;
+      pos[1] = pos[0] + 8;
+    } else {
+      pos0 = min(r0 + 63, p.Nq - 1) / p.qpos != r0 / p.qpos ? 0 : r0 % p.qpos;
+      pos[0] = (r0 + 16 * warp + lane / 4) % p.qpos;
+      pos[1] = (r0 + 16 * warp + lane / 4 + 8) % p.qpos;
+    }
+  }
+  for (int j = kv.x; j < kv.y; ++j) {
     // ---- S = Q K^T over the d-chunks
     float s[NS];
     wg_fence();
@@ -215,10 +283,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
             s[4 * jj + 2 + e] = -INFINITY;
           }
     }
-    if (kCausal && j * kBN + kBN - 1 > r0 + p.diag) {   // the block crosses the diagonal of this warpgroup's rows
-#pragma unroll
+    if (kCausal && j * kBN + kBN - 1 > (kGQA ? pos0 : r0) + p.diag) {   // the block crosses the diagonal of this
+#pragma unroll                                                          // warpgroup's rows
       for (int i = 0; i < 2; ++i) {
-        const int last = r0 + 16 * warp + lane / 4 + 8 * i + p.diag - kbase;   // last visible key, from kbase
+        // last visible key, from kbase
+        const int last = (kGQA ? pos[i] : r0 + 16 * warp + lane / 4 + 8 * i) + p.diag - kbase;
 #pragma unroll
         for (int jj = 0; jj < kBN / 8; ++jj)
 #pragma unroll
@@ -310,8 +379,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     lt += __shfl_xor_sync(0xffffffffu, lt, 1);
     lt += __shfl_xor_sync(0xffffffffu, lt, 2);
     lsum[i] = lt;
-    // an empty row is told by m, not by l: exp2_fma_pipe(-inf) = 2^-126 leaves l slightly above 0
-    inv[i] = kCausal && m[i] == -INFINITY ? 0.f : 1.f / lt;
+    // an empty row (or a split that visited no block) is told by m, not by l: exp2_fma_pipe(-inf) = 2^-126 leaves l
+    // slightly above 0
+    inv[i] = (kCausal || kSplit) && m[i] == -INFINITY ? 0.f : 1.f / lt;
     ss[i] = 0.f;
     if (p.rms_g > 0.f) {
 #pragma unroll
@@ -346,13 +416,38 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     }
     cluster_sync_all();   // no CTA leaves while a peer may still read its statistics
   }
+  if constexpr (kSplit) {
+    {   // this split's normalised O in fp32 and its lse, combined by attn_combine_kernel
+      const size_t part = static_cast<size_t>(blockIdx.z) * gridDim.y * p.Nq;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int row = q0 + 64 * w + 16 * warp + lane / 4 + 8 * i;
+        if (row >= row_end) continue;
+        if (slab == 0 && (lane % 4) == 0)
+          p.ws_lse[part + head + row] =
+              m[i] == -INFINITY ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
+        float* orow = p.ws_o + (part + head + row) * p.D;
+#pragma unroll
+        for (int c = 0; c < NDC; ++c)
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
+            if (col < p.D)
+              *reinterpret_cast<float2*>(orow + col) =
+                  make_float2(o[c][4 * jj + 2 * i] * inv[i], o[c][4 * jj + 2 * i + 1] * inv[i]);
+          }
+      }
+      return;
+    }
+  }
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     if (p.rms_g > 0.f) inv[i] *= rsqrtf(ss[i] / static_cast<float>(p.D) + 1e-5f) * p.rms_g;
     const int row = q0 + 64 * w + 16 * warp + lane / 4 + 8 * i;
-    if (row >= p.Nq) continue;
+    if (row >= (kGQA ? row_end : p.Nq)) continue;
     if (p.lse && slab == 0 && (lane % 4) == 0)
-      p.lse[head + row] = kCausal && m[i] == -INFINITY ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
+      p.lse[head + row] =
+          kCausal && m[i] == -INFINITY ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
     __half* orow = p.o_ptr + (head + row) * p.D;
 #pragma unroll
     for (int c = 0; c < NDC; ++c)

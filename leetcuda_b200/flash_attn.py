@@ -65,8 +65,9 @@ V_TRANSPOSED_OPS = {
 OP_NAMES = _BASIC + _ACC_F32 + _SWIZZLE + _OTHERS
 
 
-def _shapes(Q, K, V, O, v_transposed, same_length):
-    """(B, H, Nq, Nk, D) of q, o [B,H,Nq,D], k [B,H,Nk,D], v [B,H,Nk,D] or [B,H,D,Nk]; Nk = Nq if same_length."""
+def _shapes(Q, K, V, O, v_transposed, same_length, grouped=False):
+    """(B, H, Nq, Nk, D, Hkv) of q, o [B,H,Nq,D], k [B,Hkv,Nk,D], v [B,Hkv,Nk,D] or [B,Hkv,D,Nk]; Nk = Nq if
+    same_length; Hkv = H unless grouped, where any Hkv dividing H is accepted."""
     for t in (Q, K, V, O):
         if t.dtype != torch.float16:
             raise RuntimeError("values must be torch::kHalf")
@@ -74,12 +75,13 @@ def _shapes(Q, K, V, O, v_transposed, same_length):
         raise RuntimeError("Tensor size mismatch!")
     B, H, Nq, D = Q.shape
     Nk = Nq if same_length else K.shape[2]
-    if tuple(K.shape) != (B, H, Nk, D) or tuple(O.shape) != (B, H, Nq, D):
+    Hkv = K.shape[1] if grouped and K.shape[1] > 0 and H % K.shape[1] == 0 else H
+    if tuple(K.shape) != (B, Hkv, Nk, D) or tuple(O.shape) != (B, H, Nq, D):
         raise RuntimeError("Tensor size mismatch!")
-    want_v = (B, H, D, Nk) if v_transposed else (B, H, Nk, D)
+    want_v = (B, Hkv, D, Nk) if v_transposed else (B, Hkv, Nk, D)
     if tuple(V.shape) != want_v:
         raise RuntimeError("Tensor size mismatch!")
-    return B, H, Nq, Nk, D
+    return B, H, Nq, Nk, D, Hkv
 
 
 def _placement(*tensors):
@@ -92,26 +94,37 @@ def _placement(*tensors):
 
 def _check(Q, K, V, O, v_transposed):
     # reference: CHECK_TORCH_TENSOR_DTYPE / _SHAPE (kernels/flash-attn/utils/utils.h:137-147): one length N for all
-    B, H, N, _, D = _shapes(Q, K, V, O, v_transposed, same_length=True)
+    B, H, N, _, D, _ = _shapes(Q, K, V, O, v_transposed, same_length=True)
     _placement(Q, K, V, O)
     return B, H, N, D
 
 
-def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=None, causal: bool = False) -> None:
+def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=None, causal: bool = False,
+             num_splits: int = 1) -> None:
     """``O = softmax(Q K^T * scale) V`` on the current CUDA stream of ``Q``'s device.
 
-    Q, O are ``[B,H,Nq,D]``; K is ``[B,H,Nk,D]`` and V ``[B,H,Nk,D]`` (or ``[B,H,D,Nk]`` with ``v_transposed``), where
-    Nk may differ from Nq.  ``lse`` (optional, fp32 ``[B,H,Nq]`` CUDA tensor) receives ``ln sum_j exp(scale * q_i . k_j)``
-    per query row — the statistic ``merge_attn_states`` needs to combine results over disjoint key ranges.
+    Q, O are ``[B,H,Nq,D]``; K is ``[B,Hkv,Nk,D]`` and V ``[B,Hkv,Nk,D]`` (or ``[B,Hkv,D,Nk]`` with ``v_transposed``),
+    where Nk may differ from Nq and Hkv may be any divisor of H: grouped-query attention, query head h reading K/V head
+    ``h // (H // Hkv)`` as torch SDPA's ``enable_gqa`` does (Hkv = 1 is multi-query attention).  ``lse`` (optional,
+    fp32 ``[B,H,Nq]`` CUDA tensor) receives ``ln sum_j exp(scale * q_i . k_j)`` per query row — the statistic
+    ``merge_attn_states`` needs to combine results over disjoint key ranges.
 
     ``causal=True`` masks key j for query i when ``j > i + (Nk - Nq)``: the diagonal is aligned bottom-right as in
     FlashAttention-2 (the queries are the last Nq positions of the key sequence).  This is not torch SDPA's
-    ``is_causal`` when Nq != Nk, which aligns it top-left.  Rows with no visible key (Nq > Nk) get O = 0, lse = -inf."""
-    B, H, Nq, Nk, D = _shapes(Q, K, V, O, v_transposed, same_length=False)
+    ``is_causal`` when Nq != Nk, which aligns it top-left.  Rows with no visible key (Nq > Nk) get O = 0, lse = -inf.
+
+    ``num_splits`` cuts the keys of every CTA into that many ranges that run in parallel and are combined in fp32
+    (split-KV, ``b200_fmha_fwd_f16_gqa``): 1 (the default) does not split, 0 lets the library choose from the shapes
+    and the GPU's SM count — the choice for decoding (small Nq, long Nk), where an unsplit grid leaves most SMs idle.
+    At most ``_capi.FMHA_MAX_SPLITS``."""
+    B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, v_transposed, same_length=False, grouped=True)
+    if isinstance(num_splits, bool) or not isinstance(num_splits, int) or not 0 <= num_splits <= _capi.FMHA_MAX_SPLITS:
+        raise RuntimeError(f"leetcuda_b200.flash_attn: num_splits must be an int in 0 .. {_capi.FMHA_MAX_SPLITS}, "
+                           f"got {num_splits!r}")
     if lse is not None and (lse.dtype != torch.float32 or tuple(lse.shape) != (B, H, Nq)):
         raise RuntimeError("leetcuda_b200.flash_attn: lse must be a contiguous fp32 CUDA tensor [B,H,Nq]")
     _placement(Q, K, V, O, *(() if lse is None else (lse,)))
-    _run(Q, K, V, O, B, H, Nq, Nk, D, v_transposed, scale, lse, causal)
+    _run(Q, K, V, O, B, H, Nq, Nk, D, v_transposed, scale, lse, causal, Hkv, num_splits)
 
 
 def _fmha_one_length(Q, K, V, O, v_transposed=False) -> None:
@@ -120,10 +133,14 @@ def _fmha_one_length(Q, K, V, O, v_transposed=False) -> None:
     _run(Q, K, V, O, B, H, N, N, D, v_transposed, 0.0, None, False)
 
 
-def _run(Q, K, V, O, B, H, Nq, Nk, D, v_transposed, scale, lse, causal) -> None:
+def _run(Q, K, V, O, B, H, Nq, Nk, D, v_transposed, scale, lse, causal, Hkv=None, num_splits=1) -> None:
     idx = Q.device.index
     args = [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr()]
-    if causal or Nk != Nq:
+    if (Hkv is not None and Hkv != H) or num_splits != 1:
+        fn = _capi.lib().b200_fmha_fwd_f16_gqa
+        args += [None if lse is None else lse.data_ptr(), B, H, Hkv, Nq, Nk, D, int(v_transposed), int(bool(causal)),
+                 int(num_splits), float(scale)]
+    elif causal or Nk != Nq:
         fn = _capi.lib().b200_fmha_fwd_f16_kv
         args += [None if lse is None else lse.data_ptr(), B, H, Nq, Nk, D, int(v_transposed), int(bool(causal)),
                  float(scale)]

@@ -168,6 +168,27 @@ int b200_fmha_fwd_f16_gqa(const void* q, const void* k, const void* v, void* o, 
  * B200_E* code for a bad shape.  Depends on the shapes and the device's SM count only (not on causal or the layout). */
 int b200_fmha_fwd_f16_gqa_splits(int B, int H, int Hkv, int Nq, int Nk, int D);
 
+/* Per-sequence query and key lengths over padded buffers: batched decoding and prefill against a KV cache.
+ *
+ * q, o: [B,H,Nq,D].  k, v: [B,Hkv,Nk,D] (natural V only), e.g. a KV cache allocated for Nk positions.  lse: [B,H,Nq]
+ * fp32 or NULL.  seqlens_q, seqlens_k: int32 [B] in device memory, or NULL for Nq resp. Nk for every sequence.
+ * Sequence b has Lq_b = clamp(seqlens_q[b], 0, Nq) queries (rows 0 .. Lq_b - 1) and Lk_b = clamp(seqlens_k[b], 0, Nk)
+ * keys (rows 0 .. Lk_b - 1).  Keys at or past Lk_b contribute nothing whatever they hold (NaN, Inf, stale data); causal
+ * masking is per sequence and bottom-right: key j is masked for query i when j > i + (Lk_b - Lq_b).  Padded rows
+ * (i >= Lq_b) and rows without a visible key get O = 0 and lse = -inf, written as such even where Q holds NaN, so the
+ * output holds no uninitialised memory and b200_merge_attn_states treats those rows as empty parts.
+ * The lengths are read by the kernel only: the host neither copies them nor synchronises, so a captured CUDA graph
+ * replays correctly after new lengths are written into the same arrays.  num_splits = 0 chooses the split count from
+ * the padded shape (b200_fmha_fwd_f16_gqa_splits(B, H, Hkv, Nq, Nk, D)), not from the lengths.  GQA head mapping,
+ * scale, num_splits, the split workspace, the combine and numerics are those of b200_fmha_fwd_f16_gqa; with
+ * num_splits = 1 each sequence's rows equal b200_fmha_fwd_f16_gqa on that sequence alone (Nq = Lq_b, Nk = Lk_b), bit
+ * for bit.  Constraints: those of b200_fmha_fwd_f16_gqa (B * Hkv <= 65535, o 16-byte aligned when num_splits != 1),
+ * and the length arrays 4-byte aligned with B entries. */
+int b200_fmha_fwd_f16_seqlens(const void* q, const void* k, const void* v, void* o, float* lse /* may be NULL */,
+                              const int* seqlens_q /* may be NULL */, const int* seqlens_k /* may be NULL */,
+                              int B, int H, int Hkv, int Nq, int Nk, int D, int causal, int num_splits, float scale,
+                              void* stream);
+
 /* ------------------------------------------------------------------ SGEMM (TF32)
  * C[M,N] (fp32) = A[M,K] (fp32) x B on the tensor cores through wgmma .tf32 with fp32
  * accumulation — the sibling of the HGEMM path (SURVEY §8f-2).  Replaces

@@ -24,27 +24,21 @@ constexpr int kMaxSplits = 64;
 constexpr int kMinBlocksPerSplit = 4;
 constexpr int kMinBlocksToSplit = 16;
 
-template <int kDS, int kBN, int kWG, bool kVT>
-int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const attn::Params& p, int qtiles,
-                int BH, int smem, bool causal, bool packed, int splits, cudaStream_t stream) {
-  // packed query heads need the kGQA kernels only for the mask; a split always runs a kSplit kernel
-  auto kern = splits > 1 ? (causal ? attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true, true, true>
-                                   : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, false, false, true>)
-                         : (causal ? (packed ? attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true, true>
-                                             : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true>)
-                                   : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, false>);
-  const int variant = splits > 1 ? 3 + causal : causal + (causal && packed);
-  static int attr_smem[5][64] = {};
+// One attention kernel on a grid of (query tiles x slabs, K/V heads, splits); attr_smem[dev] remembers the dynamic
+// shared memory the kernel was allowed on each device.
+template <typename... Params, typename... Args>
+int launch_kernel(void (*kern)(Params...), int* attr_smem, const attn::Params& p, int qtiles, int BH, int splits,
+                  int threads, int smem, cudaStream_t stream, const Args&... args) {
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && attr_smem[variant][dev] < smem) {
+  if (dev >= 0 && dev < 64 && attr_smem[dev] < smem) {
     B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_smem[variant][dev] = smem;
+    attr_smem[dev] = smem;
   }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(static_cast<unsigned>(qtiles * p.slabs), static_cast<unsigned>(BH), static_cast<unsigned>(splits));
-  cfg.blockDim = dim3(attn::threads<kWG>(), 1, 1);
+  cfg.blockDim = dim3(threads, 1, 1);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
   cudaLaunchAttribute attrs[1];
@@ -54,9 +48,36 @@ int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap&
   attrs[0].val.clusterDim.z = 1;
   cfg.attrs = attrs;
   cfg.numAttrs = 1;
-  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tq, tk, tv, p));
+  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, args...));
   host::count_launch();
   return 0;
+}
+
+// lens != nullptr: per-sequence lengths, attn_fwd_seqlens_kernel (natural V only)
+template <int kDS, int kBN, int kWG, bool kVT>
+int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const attn::Params& p, int qtiles,
+                int BH, int smem, bool causal, bool packed, int splits, const attn::Lens* lens, cudaStream_t stream) {
+  if constexpr (!kVT) {
+    if (lens != nullptr) {
+      auto kern = splits > 1 ? (causal ? attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, true, true>
+                                       : attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, false, true>)
+                             : (causal ? attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, true, false>
+                                       : attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, false, false>);
+      static int attr_smem[4][64] = {};
+      return launch_kernel(kern, attr_smem[2 * (splits > 1) + causal], p, qtiles, BH, splits, attn::threads<kWG>(),
+                           smem, stream, tq, tk, tv, p, *lens);
+    }
+  }
+  // packed query heads need the kGQA kernels only for the mask; a split always runs a kSplit kernel
+  auto kern = splits > 1 ? (causal ? attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true, true, true>
+                                   : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, false, false, true>)
+                         : (causal ? (packed ? attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true, true>
+                                             : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true>)
+                                   : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, false>);
+  const int variant = splits > 1 ? 3 + causal : causal + (causal && packed);
+  static int attr_smem[5][64] = {};
+  return launch_kernel(kern, attr_smem[variant], p, qtiles, BH, splits, attn::threads<kWG>(), smem, stream, tq, tk, tv,
+                       p);
 }
 
 // [BH, D, N] -> [BH, N, D] (fp16): the three reference ops that take V pre-transposed
@@ -149,7 +170,7 @@ Family family(int D) {
 // splits whose fp32 parts go to ws_o / ws_lse instead of o / lse (kSplit kernels).  Causal with G > 1 runs kGQA.
 int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int Hkv, int G,
                   int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, float* ws_o, float* ws_lse,
-                  cudaStream_t stream) {
+                  cudaStream_t stream, const attn::Lens* lens = nullptr) {
   const uint64_t BH = static_cast<uint64_t>(B) * Hkv;
   const Family f = family(D);
   const int ds = f.ds, bn = f.bn, wgs = f.wgs;
@@ -202,26 +223,31 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
     if ((rc = host::get_tmap(&tv, v, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   }
   const int bh = static_cast<int>(BH);
-  if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, G > 1, splits, stream)
-                          : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, G > 1, splits, stream);
-  if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, G > 1, splits, stream)
-                           : launch_attn<128, 64, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, G > 1, splits, stream);
+  if (vt && lens) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with lengths)");
+  const bool pk = G > 1;
+  if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, stream)
+                          : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, stream);
+  if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, stream)
+                           : launch_attn<128, 64, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, stream);
   if (vt) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with D=%d)", D);
-  return launch_attn<256, 64, 1, false>(tq, tk, tv, p, qtiles, bh, smem, causal, G > 1, splits, stream);
+  return launch_attn<256, 64, 1, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, stream);
 }
 
 // The attention kernel, and with splits > 1 its fp32 parts in a stream-ordered workspace and the combine kernel.
 int fmha_run(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int Hkv, int G,
-             int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, cudaStream_t stream) {
+             int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, cudaStream_t stream,
+             const attn::Lens* lens = nullptr) {
   if (splits <= 1)
-    return fmha_dispatch(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, 1, nullptr, nullptr, stream);
+    return fmha_dispatch(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, 1, nullptr, nullptr, stream,
+                         lens);
   const size_t rows = static_cast<size_t>(B) * Hkv * G * Nq;
   const size_t lse_bytes = (static_cast<size_t>(splits) * rows * 4 + 255) & ~static_cast<size_t>(255);
   void* ws = nullptr;
   B200_CUDA_OK(cudaMallocAsync(&ws, lse_bytes + static_cast<size_t>(splits) * rows * D * 4, stream));
   float* ws_lse = static_cast<float*>(ws);
   float* ws_o = reinterpret_cast<float*>(static_cast<char*>(ws) + lse_bytes);
-  int rc = fmha_dispatch(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, splits, ws_o, ws_lse, stream);
+  int rc = fmha_dispatch(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, splits, ws_o, ws_lse, stream,
+                         lens);
   if (rc == 0) rc = launch_combine(static_cast<__half*>(o), lse, ws_o, ws_lse, rows, D, splits, stream);
   cudaFreeAsync(ws, stream);
   return rc;
@@ -347,6 +373,41 @@ int b200_fmha_fwd_f16_gqa_splits(int B, int H, int Hkv, int Nq, int Nk, int D) {
   if (Hkv <= 0 || H % Hkv != 0)
     return fail(B200_EINVAL, "fmha_gqa_splits: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
   return auto_splits(B, Hkv, H / Hkv, Nq, Nk, D);
+}
+
+int b200_fmha_fwd_f16_seqlens(const void* q, const void* k, const void* v, void* o, float* lse, const int* seqlens_q,
+                              const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk, int D, int causal,
+                              int num_splits, float scale, void* stream) {
+  if (!q || !k || !v || !o) return fail(B200_EINVAL, "fmha_seqlens: null pointer (q, k, v and o are required)");
+  if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "fmha_seqlens: bad shape B=%d H=%d D=%d", B, H, D);
+  if (Nq <= 0 || Nk <= 0)
+    return fail(B200_EINVAL, "fmha_seqlens: bad lengths Nq=%d Nk=%d (both must be >= 1)", Nq, Nk);
+  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_seqlens: causal must be 0 or 1, got %d", causal);
+  if (Hkv <= 0 || H % Hkv != 0)
+    return fail(B200_EINVAL, "fmha_seqlens: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
+  if (num_splits < 0 || num_splits > kMaxSplits)
+    return fail(B200_EINVAL, "fmha_seqlens: num_splits=%d must be in 0 .. %d", num_splits, kMaxSplits);
+  if (static_cast<long long>(B) * Hkv > 65535)
+    return fail(B200_EINVAL, "fmha_seqlens: B*Hkv = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
+  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
+    return fail(B200_EINVAL,
+                "fmha_seqlens: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)");
+  if (static_cast<long long>(H / Hkv) * Nq > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "fmha_seqlens: (H/Hkv)*Nq = %lld query rows per K/V head exceed 2^31 - 1",
+                static_cast<long long>(H / Hkv) * Nq);
+  if ((reinterpret_cast<uintptr_t>(seqlens_q) & 3u) != 0)
+    return fail(B200_EINVAL, "fmha_seqlens: seqlens_q must be 4-byte aligned (int32)");
+  if ((reinterpret_cast<uintptr_t>(seqlens_k) & 3u) != 0)
+    return fail(B200_EINVAL, "fmha_seqlens: seqlens_k must be 4-byte aligned (int32)");
+  if (D % 8 != 0) return fail(B200_ENOTSUP, "fmha_seqlens: headdim not support! (D=%d must be a multiple of 8)", D);
+  if (D > 1024) return fail(B200_ENOTSUP, "fmha_seqlens: headdim not support! (D=%d > 1024)", D);
+  if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
+  const int G = H / Hkv;
+  // the split count follows the padded shape, as for b200_fmha_fwd_f16_gqa: the lengths stay on the device
+  const int splits = num_splits == 0 ? auto_splits(B, Hkv, G, Nq, Nk, D) : num_splits;
+  const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
+  return fmha_run(q, k, v, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
+                  static_cast<cudaStream_t>(stream), &lens);
 }
 
 int b200_fmha_fwd_f16_rmsnorm(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H,

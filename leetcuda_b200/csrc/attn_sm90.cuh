@@ -36,6 +36,15 @@
 //     holds the rows of several heads.
 //   * kSplit: grid.z cuts the key blocks [0, nkv) a CTA visits into contiguous ranges; the epilogue writes the
 //     split's normalised O in fp32 and its lse to a workspace that a combine kernel reduces.
+//
+// Per-sequence lengths (attn_fwd_seqlens_kernel, b200_fmha_fwd_f16_seqlens): Q and K/V are padded to Nq and Nk, and
+// sequence b has Lq_b <= Nq queries and Lk_b <= Nk keys, read from device arrays by every CTA before it starts.
+//   * a CTA runs with Nk = Lk_b, diag = Lk_b - Lq_b and the key blocks of Lk_b; packed row r has position r % Nq (for
+//     every G, causal or not) and is a padded row when that position is >= Lq_b; a causal tile visits the blocks left
+//     of the diagonal of its greatest valid position, a tile of padded rows none;
+//   * keys >= Lk_b are masked like the tail past Nk; V rows >= Lk_b of the one partial key block are zeroed in shared
+//     memory (producer warp 1) before the consumers read them, since P = 0 times a NaN or Inf of V is NaN;
+//   * padded rows and rows without a visible key store O = 0 and lse = -inf as literal values.
 #pragma once
 #include <cuda.h>
 
@@ -61,6 +70,14 @@ struct Params {
   int qpos;            // kGQA: query positions per head (the call's Nq); packed row r has position r % qpos
   int tph;             // kGQA: > 0: every query head has its own tph tiles (no tile straddles two heads), 0: the
                        // tiles cut the packed rows of the group
+};
+
+// attn_fwd_seqlens_kernel: the per-sequence lengths (int32 [B] on the device, or nullptr for Nq / Nk) and the K/V heads
+// per sequence (grid.y = b * hkv + K/V head)
+struct Lens {
+  const int* q;
+  const int* k;
+  int hkv;
 };
 
 // Keys whose exponential the D <= 128 kernels evaluate on the FMA pipe (exp2_fma_pipe) instead of MUFU.EX2: bit i
@@ -98,10 +115,26 @@ __device__ __forceinline__ int causal_kv_blocks(const Params& p, int rows_end, i
 // query position (kGQA: of a packed row), with kSplit the grid.z-th of gridDim.z contiguous ranges of them (possibly
 // empty).  The producer and the consumers both take their loop bounds from here.
 // kGQA: the CTA's rows [q0, row_end) are query positions from q0 - off on (per-head tiles), or packed rows (p.tph = 0).
-template <int kBN, int kRows, bool kCausal, bool kGQA, bool kSplit>
-__device__ __forceinline__ int2 kv_blocks(const Params& p, int q0, int row_end, int off) {
+// kSeqlens: p holds the sequence's Lk and diag, and only the positions below lq count; a tile without one visits no
+// block.  A packed tile that crosses into the next query head holds position 0 and is taken to reach lq - 1.
+template <int kBN, int kRows, bool kCausal, bool kGQA, bool kSplit, bool kSeqlens = false>
+__device__ __forceinline__ int2 kv_blocks(const Params& p, int q0, int row_end, int off, int lq = 0) {
   int nkv = p.num_kv;
-  if constexpr (kCausal) {
+  if constexpr (kSeqlens) {
+    int first, end;   // the tile's query positions [first, end)
+    if (p.tph > 0) {
+      first = q0 - off;
+      end = min(q0 + kRows, row_end) - off;
+    } else {
+      const int last = min(q0 + kRows, p.Nq) - 1;
+      const bool cross = last / p.qpos != q0 / p.qpos;
+      first = cross ? 0 : q0 % p.qpos;
+      end = cross ? p.qpos : last % p.qpos + 1;
+    }
+    end = min(end, lq);
+    if (end <= first) nkv = 0;
+    else if (kCausal) nkv = causal_kv_blocks(p, end, kBN);
+  } else if constexpr (kCausal) {
     int rows_end = q0 + kRows;
     if constexpr (kGQA) {
       if (p.tph > 0) {
@@ -122,13 +155,14 @@ __device__ __forceinline__ int2 kv_blocks(const Params& p, int q0, int row_end, 
 }
 
 // kDS: columns of O per CTA (64, 128 or 256); kBN: keys per block; kVT: V is [B,H,D,N]; kCausal: the causal mask;
-// kGQA: the causal mask on packed query heads; kSplit: split-KV (see the top of this file).
-// kCausal, kGQA and kSplit are template parameters so that the other kernels compile to the code they had without them.
-template <int kDS, int kBN, int kWG, bool kVT, bool kCausal, bool kGQA = false, bool kSplit = false>
-__global__ void __launch_bounds__(threads<kWG>(), 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                const __grid_constant__ CUtensorMap tmap_v, const Params p) {
+// kGQA: the causal mask on packed query heads; kSplit: split-KV; kSeqlens: per-sequence lengths from `lens` (see the top
+// of this file).  kCausal, kGQA, kSplit and kSeqlens are template parameters so that the other kernels compile to the
+// code they had without them.
+template <int kDS, int kBN, int kWG, bool kVT, bool kCausal, bool kGQA, bool kSplit, bool kSeqlens>
+__device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k,
+                                              const CUtensorMap& tmap_v, Params p, const Lens& lens) {
   static_assert(!kVT || kDS <= 128, "transposed V: one slab of <= 128 columns");
+  static_assert(!kSeqlens || (!kVT && kGQA), "per-sequence lengths: natural V, query positions of packed rows");
   constexpr int SLOT = slot_bytes(kBN, kDS, kVT);
   constexpr int KV_BYTES = 64 * kBN * 2;   // one {64 columns, kBN keys} chunk of K or V
   constexpr int NS = kBN / 2;     // S accumulator registers per thread
@@ -164,9 +198,27 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   const int slab = blockIdx.x % p.slabs;
   const int bh = blockIdx.y;
   const int d0 = slab * kDS;
-  const int2 kv = kv_blocks<kBN, 64 * kWG, kCausal, kGQA, kSplit>(p, q0, row_end, off);
+  // kSeqlens: this sequence's valid query positions lq and keys p.Nk (nk_pad: the padded Nk of the K/V buffers)
+  int lq = 0;
+  [[maybe_unused]] const int nk_pad = p.Nk;
+  if constexpr (kSeqlens) {
+    const int b = blockIdx.y / lens.hkv;
+    lq = lens.q ? min(max(__ldg(lens.q + b), 0), p.qpos) : p.qpos;
+    const int lk = lens.k ? min(max(__ldg(lens.k + b), 0), nk_pad) : nk_pad;
+    p.Nk = lk;
+    p.diag = lk - lq;
+    p.num_kv = (lk + kBN - 1) / kBN;
+  }
+  const int2 kv = kv_blocks<kBN, 64 * kWG, kCausal, kGQA, kSplit, kSeqlens>(p, q0, row_end, off, lq);
   // V chunks of this slab per key block
   const int nvc = kVT ? kBN / 64 : min(NDC, (p.D - d0 + 63) / 64);
+  // kSeqlens: the visited key block that ends past Lk_b inside the K/V buffers (-1: none).  TMA zero-fills only past
+  // nk_pad, so its V rows of keys >= Lk_b are zeroed in shared memory before the consumers read them.
+  [[maybe_unused]] int vz = -1;
+  [[maybe_unused]] const uint32_t vbar = rowss;   // its V chunks land here (no fused RMS norm with kSeqlens)
+  if constexpr (kSeqlens) {
+    if (p.Nk % kBN != 0 && p.Nk < nk_pad && p.num_kv - 1 >= kv.x && p.num_kv - 1 < kv.y) vz = p.num_kv - 1;
+  }
 
   if (threadIdx.x == 0) {
     mbar_init(qbar, 1);
@@ -174,6 +226,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       mbar_init(full(s), 1);
       mbar_init(empty(s), 4 * kWG);   // lane 0 of every consumer warp
     }
+    if constexpr (kSeqlens) mbar_init(vbar, 1);
     fence_mbar_init();
   }
   __syncthreads();
@@ -206,10 +259,39 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
             const int s = next(64 * kDS * 2);
             tma_load_3d(sring + s * SLOT, &tmap_v, full(s), j * kBN + 64 * c, d0, bh, kEvictLast);
           } else {
+            if constexpr (kSeqlens) {
+              if (j == vz) {
+                // onto vbar, not the slot's full barrier: warp 1 arrives there once the rows past Lk_b are zero
+                const int s = it % p.ring;
+                if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
+                ++it;
+                if (c == 0) mbar_expect_tx(vbar, nvc * KV_BYTES);
+                tma_load_3d(sring + s * SLOT, &tmap_v, vbar, d0 + 64 * c, j * kBN, bh, kEvictLast);
+                continue;
+              }
+            }
             const int s = next(KV_BYTES);
             tma_load_3d(sring + s * SLOT, &tmap_v, full(s), d0 + 64 * c, j * kBN, bh, kEvictLast);
           }
         }
+      }
+    }
+    if constexpr (kSeqlens) {
+      if (tid / 32 == 1 && vz >= 0) {
+        // a natural-V chunk {64 d, kBN keys} holds key r in the 128-byte row r (the 128B swizzle permutes 16-byte units
+        // within a row only): zero rows Lk_b - vz * kBN .. kBN - 1 of the block's V chunks, then publish them
+        const int it0 = (vz - kv.x) * (p.nq + nvc) + p.nq;   // the producer's slot count at the block's first V chunk
+        const int zb = (p.Nk - vz * kBN) * 128;
+        mbar_wait(vbar, 0);
+        for (int c = 0; c < nvc; ++c) {
+          uint8_t* chunk = smem + (sring - sq) + ((it0 + c) % p.ring) * SLOT;
+          for (int x = zb + 16 * (tid % 32); x < kBN * 128; x += 512)
+            *reinterpret_cast<uint4*>(chunk + x) = make_uint4(0u, 0u, 0u, 0u);
+        }
+        fence_proxy_async_smem();   // the consumers' wgmma reads V through the async proxy
+        __syncwarp();
+        if (tid % 32 == 0)
+          for (int c = 0; c < nvc; ++c) mbar_arrive(full((it0 + c) % p.ring));
       }
     }
     if (rms_cluster) {   // the consumers' two cluster barriers (epilogue)
@@ -304,8 +386,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       const float mn = fmaxf(m[i], mx * p.scale_log2);
-      // a row without a visible key so far (causal only): subtract 0, so that alpha and x are exp2(-inf), not NaN
-      const float mb = kCausal && mn == -INFINITY ? 0.f : mn;
+      // a row without a visible key so far (causal or per-sequence lengths only): subtract 0, so that alpha and x are
+      // exp2(-inf), not NaN
+      const float mb = (kCausal || kSeqlens) && mn == -INFINITY ? 0.f : mn;
       alpha[i] = fast_exp2(m[i] - mb);
       m[i] = mn;
       float sum = 0.f;
@@ -381,7 +464,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     lsum[i] = lt;
     // an empty row (or a split that visited no block) is told by m, not by l: exp2_fma_pipe(-inf) = 2^-126 leaves l
     // slightly above 0
-    inv[i] = (kCausal || kSplit) && m[i] == -INFINITY ? 0.f : 1.f / lt;
+    inv[i] = (kCausal || kSplit || kSeqlens) && m[i] == -INFINITY ? 0.f : 1.f / lt;
     ss[i] = 0.f;
     if (p.rms_g > 0.f) {
 #pragma unroll
@@ -423,9 +506,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       for (int i = 0; i < 2; ++i) {
         const int row = q0 + 64 * w + 16 * warp + lane / 4 + 8 * i;
         if (row >= row_end) continue;
+        // kSeqlens: a padded row is an empty part (a select: o * inv may be NaN there)
+        const bool pad = kSeqlens && (p.tph > 0 ? row - off : row % p.qpos) >= lq;
         if (slab == 0 && (lane % 4) == 0)
           p.ws_lse[part + head + row] =
-              m[i] == -INFINITY ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
+              m[i] == -INFINITY || pad ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
         float* orow = p.ws_o + (part + head + row) * p.D;
 #pragma unroll
         for (int c = 0; c < NDC; ++c)
@@ -434,7 +519,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
             const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
             if (col < p.D)
               *reinterpret_cast<float2*>(orow + col) =
-                  make_float2(o[c][4 * jj + 2 * i] * inv[i], o[c][4 * jj + 2 * i + 1] * inv[i]);
+                  make_float2(pad ? 0.f : o[c][4 * jj + 2 * i] * inv[i], pad ? 0.f : o[c][4 * jj + 2 * i + 1] * inv[i]);
           }
       }
       return;
@@ -445,6 +530,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     if (p.rms_g > 0.f) inv[i] *= rsqrtf(ss[i] / static_cast<float>(p.D) + 1e-5f) * p.rms_g;
     const int row = q0 + 64 * w + 16 * warp + lane / 4 + 8 * i;
     if (row >= (kGQA ? row_end : p.Nq)) continue;
+    if constexpr (kSeqlens) {
+      // a padded row, or one without a visible key: literal 0 and -inf (o * inv may be NaN in a padded row)
+      if ((p.tph > 0 ? row - off : row % p.qpos) >= lq || m[i] == -INFINITY) {
+        if (p.lse && slab == 0 && (lane % 4) == 0) p.lse[head + row] = -INFINITY;
+#pragma unroll
+        for (int c = 0; c < NDC; ++c)
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
+            if (col < p.D) *reinterpret_cast<uint32_t*>(p.o_ptr + (head + row) * p.D + col) = 0u;
+          }
+        continue;
+      }
+    }
     if (p.lse && slab == 0 && (lane % 4) == 0)
       p.lse[head + row] =
           kCausal && m[i] == -INFINITY ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
@@ -459,6 +558,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
               pack_half2(o[c][4 * jj + 2 * i] * inv[i], o[c][4 * jj + 2 * i + 1] * inv[i]);
       }
   }
+}
+
+template <int kDS, int kBN, int kWG, bool kVT, bool kCausal, bool kGQA = false, bool kSplit = false>
+__global__ void __launch_bounds__(threads<kWG>(), 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                const __grid_constant__ CUtensorMap tmap_v, const Params p) {
+  attn_fwd_body<kDS, kBN, kWG, kVT, kCausal, kGQA, kSplit, false>(tmap_q, tmap_k, tmap_v, p, Lens{});
+}
+
+// Per-sequence lengths (b200_fmha_fwd_f16_seqlens): natural V, query positions of packed rows for every G.
+template <int kDS, int kBN, int kWG, bool kCausal, bool kSplit>
+__global__ void __launch_bounds__(threads<kWG>(), 1)
+attn_fwd_seqlens_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                        const __grid_constant__ CUtensorMap tmap_v, const Params p, const Lens lens) {
+  attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, kSplit, true>(tmap_q, tmap_k, tmap_v, p, lens);
 }
 
 }  // namespace attn

@@ -48,6 +48,10 @@ B200_DEVICE void fence_mbar_init() {
   // make mbarrier inits visible to the async proxy / other CTAs of the cluster
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
+B200_DEVICE void fence_proxy_async_smem() {
+  // order this thread's generic-proxy writes to shared memory before later async-proxy reads (wgmma, TMA)
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
 B200_DEVICE void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes)
                : "memory");

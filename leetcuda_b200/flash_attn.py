@@ -100,7 +100,7 @@ def _check(Q, K, V, O, v_transposed):
 
 
 def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=None, causal: bool = False,
-             num_splits: int = 1) -> None:
+             num_splits: int = 1, seqlens_q=None, seqlens_k=None) -> None:
     """``O = softmax(Q K^T * scale) V`` on the current CUDA stream of ``Q``'s device.
 
     Q, O are ``[B,H,Nq,D]``; K is ``[B,Hkv,Nk,D]`` and V ``[B,Hkv,Nk,D]`` (or ``[B,Hkv,D,Nk]`` with ``v_transposed``),
@@ -116,7 +116,17 @@ def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=
     ``num_splits`` cuts the keys of every CTA into that many ranges that run in parallel and are combined in fp32
     (split-KV, ``b200_fmha_fwd_f16_gqa``): 1 (the default) does not split, 0 lets the library choose from the shapes
     and the GPU's SM count — the choice for decoding (small Nq, long Nk), where an unsplit grid leaves most SMs idle.
-    At most ``_capi.FMHA_MAX_SPLITS``."""
+    At most ``_capi.FMHA_MAX_SPLITS``.
+
+    ``seqlens_q`` / ``seqlens_k`` (int32 contiguous CUDA tensors ``[B]`` on Q's device) give every sequence its own
+    number of queries and keys inside the padded Q / K / V (``b200_fmha_fwd_f16_seqlens``): sequence b uses query rows
+    ``0 .. clamp(seqlens_q[b], 0, Nq) - 1`` and key rows ``0 .. clamp(seqlens_k[b], 0, Nk) - 1``; keys past that
+    contribute nothing whatever they hold, the causal diagonal is per sequence, and padded query rows get O = 0,
+    lse = -inf.  The lengths are read on the GPU only (no host synchronisation), so a captured CUDA graph replays with
+    whatever lengths the tensors hold.  None means Nq resp. Nk for every sequence; natural V only."""
+    if seqlens_q is not None or seqlens_k is not None:
+        _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k)
+        return
     B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, v_transposed, same_length=False, grouped=True)
     if isinstance(num_splits, bool) or not isinstance(num_splits, int) or not 0 <= num_splits <= _capi.FMHA_MAX_SPLITS:
         raise RuntimeError(f"leetcuda_b200.flash_attn: num_splits must be an int in 0 .. {_capi.FMHA_MAX_SPLITS}, "
@@ -125,6 +135,39 @@ def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=
         raise RuntimeError("leetcuda_b200.flash_attn: lse must be a contiguous fp32 CUDA tensor [B,H,Nq]")
     _placement(Q, K, V, O, *(() if lse is None else (lse,)))
     _run(Q, K, V, O, B, H, Nq, Nk, D, v_transposed, scale, lse, causal, Hkv, num_splits)
+
+
+def _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k) -> None:
+    if v_transposed:
+        raise RuntimeError("leetcuda_b200.flash_attn: seqlens_q / seqlens_k take natural V [B,Hkv,Nk,D] only "
+                           "(v_transposed=True is not supported with lengths)")
+    B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, False, same_length=False, grouped=True)
+    if isinstance(num_splits, bool) or not isinstance(num_splits, int) or not 0 <= num_splits <= _capi.FMHA_MAX_SPLITS:
+        raise RuntimeError(f"leetcuda_b200.flash_attn: num_splits must be an int in 0 .. {_capi.FMHA_MAX_SPLITS}, "
+                           f"got {num_splits!r}")
+    if lse is not None and (lse.dtype != torch.float32 or tuple(lse.shape) != (B, H, Nq)):
+        raise RuntimeError("leetcuda_b200.flash_attn: lse must be a contiguous fp32 CUDA tensor [B,H,Nq]")
+    for name, t in (("seqlens_q", seqlens_q), ("seqlens_k", seqlens_k)):
+        if t is None:
+            continue
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or tuple(t.shape) != (B,) or not t.is_cuda \
+                or not t.is_contiguous() or t.device != Q.device:
+            raise RuntimeError(f"leetcuda_b200.flash_attn: {name} must be an int32 contiguous CUDA tensor [B] = [{B}] "
+                               f"on Q's device")
+    _placement(Q, K, V, O, *(() if lse is None else (lse,)))
+    idx = Q.device.index
+    args = [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), None if lse is None else lse.data_ptr(),
+            None if seqlens_q is None else seqlens_q.data_ptr(), None if seqlens_k is None else seqlens_k.data_ptr(),
+            B, H, Hkv, Nq, Nk, D, int(bool(causal)), int(num_splits), float(scale)]
+    fn = _capi.lib().b200_fmha_fwd_f16_seqlens
+    if torch.cuda.current_device() != idx:
+        with torch.cuda.device(idx):
+            rc = fn(*args, _capi.raw_stream(idx))
+    else:
+        rc = fn(*args, _capi.raw_stream(idx))
+    if rc == -3:
+        raise RuntimeError("headdim not support!")
+    _capi.check(rc, "fmha_fwd")
 
 
 def _fmha_one_length(Q, K, V, O, v_transposed=False) -> None:

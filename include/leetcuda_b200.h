@@ -189,6 +189,30 @@ int b200_fmha_fwd_f16_seqlens(const void* q, const void* k, const void* v, void*
                               int B, int H, int Hkv, int Nq, int Nk, int D, int causal, int num_splits, float scale,
                               void* stream);
 
+/* Paged KV cache: b200_fmha_fwd_f16_seqlens with K and V kept in a pool of fixed-size pages and a block table per
+ * sequence (the layout of FlashAttention's block-table API and of vLLM's flash-attn backend).
+ *
+ * q, o: [B,H,Nq,D].  k_cache, v_cache: each [num_pages, page_size, Hkv, D] fp16, contiguous.  block_table: int32
+ * [B, max_pages_per_seq], contiguous, in device memory.  Key t of sequence b is row t % page_size of page
+ * block_table[b][t / page_size].  Everything else is b200_fmha_fwd_f16_seqlens with the padded
+ * Nk = max_pages_per_seq * page_size: the length clamps, the per-sequence bottom-right causal mask, O = 0 and
+ * lse = -inf in padded rows and rows without a key, the GQA mapping, num_splits (0 chooses from the padded shape),
+ * the split workspace, the combine and the numerics.  With the same data, O and lse equal those of
+ * b200_fmha_fwd_f16_seqlens on a contiguous padded cache, bit for bit.
+ * Table entries at or past a sequence's last used page, ceil(Lk_b / page_size), are never read: callers may pad the
+ * table with -1 or stale ids.  Pages may be shared between sequences (prefix sharing); the pool is only read.  A page
+ * id is only ever a TMA coordinate, bounds-checked against the pool: a used entry outside [0, num_pages) gives wrong
+ * values for that sequence, never an out-of-bounds access.  The table and the lengths are read by the kernel only, so
+ * a captured CUDA graph replays correctly after new tables or lengths are written into the same arrays.
+ * Constraints: those of b200_fmha_fwd_f16_seqlens; page_size a power of two >= 16; num_pages >= 1,
+ * max_pages_per_seq >= 1; num_pages * page_size and max_pages_per_seq * page_size <= 2^31 - 1; block_table 4-byte
+ * aligned. */
+int b200_fmha_fwd_f16_paged(const void* q, const void* k_cache, const void* v_cache, void* o,
+                            float* lse /* may be NULL */, const int* block_table,
+                            const int* seqlens_q /* may be NULL */, const int* seqlens_k /* may be NULL */, int B,
+                            int H, int Hkv, int Nq, int num_pages, int page_size, int max_pages_per_seq, int D,
+                            int causal, int num_splits, float scale, void* stream);
+
 /* ------------------------------------------------------------------ SGEMM (TF32)
  * C[M,N] (fp32) = A[M,K] (fp32) x B on the tensor cores through wgmma .tf32 with fp32
  * accumulation — the sibling of the HGEMM path (SURVEY §8f-2).  Replaces

@@ -53,11 +53,22 @@ int launch_kernel(void (*kern)(Params...), int* attr_smem, const attn::Params& p
   return 0;
 }
 
-// lens != nullptr: per-sequence lengths, attn_fwd_seqlens_kernel (natural V only)
+// lens != nullptr: per-sequence lengths, attn_fwd_seqlens_kernel (natural V only); with pages also: paged K/V,
+// attn_fwd_paged_kernel
 template <int kDS, int kBN, int kWG, bool kVT>
 int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const attn::Params& p, int qtiles,
-                int BH, int smem, bool causal, bool packed, int splits, const attn::Lens* lens, cudaStream_t stream) {
+                int BH, int smem, bool causal, bool packed, int splits, const attn::Lens* lens,
+                const attn::Pages* pages, cudaStream_t stream) {
   if constexpr (!kVT) {
+    if (lens != nullptr && pages != nullptr) {
+      auto kern = splits > 1 ? (causal ? attn::attn_fwd_paged_kernel<kDS, kBN, kWG, true, true>
+                                       : attn::attn_fwd_paged_kernel<kDS, kBN, kWG, false, true>)
+                             : (causal ? attn::attn_fwd_paged_kernel<kDS, kBN, kWG, true, false>
+                                       : attn::attn_fwd_paged_kernel<kDS, kBN, kWG, false, false>);
+      static int attr_smem[4][64] = {};
+      return launch_kernel(kern, attr_smem[2 * (splits > 1) + causal], p, qtiles, BH, splits, attn::threads<kWG>(),
+                           smem, stream, tq, tk, tv, p, *lens, *pages);
+    }
     if (lens != nullptr) {
       auto kern = splits > 1 ? (causal ? attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, true, true>
                                        : attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, false, true>)
@@ -168,9 +179,11 @@ Family family(int D) {
 
 // G: query heads per K/V head (H = G * Hkv; the kernel sees B * Hkv heads of G * Nq packed rows).  splits > 1: grid.z
 // splits whose fp32 parts go to ws_o / ws_lse instead of o / lse (kSplit kernels).  Causal with G > 1 runs kGQA.
+// pages: k and v are pools of num_pages pages [page_size, Hkv, D], and Nk is the padded max_pages * page_size.
 int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int Hkv, int G,
                   int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, float* ws_o, float* ws_lse,
-                  cudaStream_t stream, const attn::Lens* lens = nullptr) {
+                  cudaStream_t stream, const attn::Lens* lens = nullptr, const attn::Pages* pages = nullptr,
+                  int num_pages = 0) {
   const uint64_t BH = static_cast<uint64_t>(B) * Hkv;
   const Family f = family(D);
   const int ds = f.ds, bn = f.bn, wgs = f.wgs;
@@ -213,33 +226,44 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
   uint32_t kbox[3] = {64, static_cast<uint32_t>(bn), 1};
   int rc;
   if ((rc = host::get_tmap(&tq, q, 3, qdims, qstr, qbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = host::get_tmap(&tk, k, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if (vt) {
-    uint64_t vd[3] = {static_cast<uint64_t>(Nk), static_cast<uint64_t>(D), BH};
-    uint64_t vs[2] = {static_cast<uint64_t>(Nk) * 2, static_cast<uint64_t>(Nk) * D * 2};
-    uint32_t vb[3] = {64, static_cast<uint32_t>(ds), 1};
-    if ((rc = host::get_tmap(&tv, v, 3, vd, vs, vb, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if (pages) {
+    // pool rows {D, Hkv, num_pages * page_size}; a key block is kBN / R boxes of R = min(page_size, kBN) rows
+    uint64_t pd[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(Hkv),
+                      static_cast<uint64_t>(num_pages) * static_cast<uint64_t>(pages->page_size)};
+    uint64_t pstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(Hkv) * D * 2};
+    uint32_t pbox[3] = {64, 1, static_cast<uint32_t>(std::min(pages->page_size, bn))};
+    if ((rc = host::get_tmap(&tk, k, 3, pd, pstr, pbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    if ((rc = host::get_tmap(&tv, v, 3, pd, pstr, pbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   } else {
-    if ((rc = host::get_tmap(&tv, v, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    if ((rc = host::get_tmap(&tk, k, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    if (vt) {
+      uint64_t vd[3] = {static_cast<uint64_t>(Nk), static_cast<uint64_t>(D), BH};
+      uint64_t vs[2] = {static_cast<uint64_t>(Nk) * 2, static_cast<uint64_t>(Nk) * D * 2};
+      uint32_t vb[3] = {64, static_cast<uint32_t>(ds), 1};
+      if ((rc = host::get_tmap(&tv, v, 3, vd, vs, vb, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    } else {
+      if ((rc = host::get_tmap(&tv, v, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    }
   }
   const int bh = static_cast<int>(BH);
   if (vt && lens) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with lengths)");
   const bool pk = G > 1;
-  if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, stream)
-                          : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, stream);
-  if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, stream)
-                           : launch_attn<128, 64, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, stream);
+  const attn::Pages* pg = pages;
+  if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream)
+                          : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream);
+  if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream)
+                           : launch_attn<128, 64, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream);
   if (vt) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with D=%d)", D);
-  return launch_attn<256, 64, 1, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, stream);
+  return launch_attn<256, 64, 1, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream);
 }
 
 // The attention kernel, and with splits > 1 its fp32 parts in a stream-ordered workspace and the combine kernel.
 int fmha_run(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int Hkv, int G,
              int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, cudaStream_t stream,
-             const attn::Lens* lens = nullptr) {
+             const attn::Lens* lens = nullptr, const attn::Pages* pages = nullptr, int num_pages = 0) {
   if (splits <= 1)
     return fmha_dispatch(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, 1, nullptr, nullptr, stream,
-                         lens);
+                         lens, pages, num_pages);
   const size_t rows = static_cast<size_t>(B) * Hkv * G * Nq;
   const size_t lse_bytes = (static_cast<size_t>(splits) * rows * 4 + 255) & ~static_cast<size_t>(255);
   void* ws = nullptr;
@@ -247,7 +271,7 @@ int fmha_run(const void* q, const void* k, const void* v, void* o, float* lse, f
   float* ws_lse = static_cast<float*>(ws);
   float* ws_o = reinterpret_cast<float*>(static_cast<char*>(ws) + lse_bytes);
   int rc = fmha_dispatch(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, splits, ws_o, ws_lse, stream,
-                         lens);
+                         lens, pages, num_pages);
   if (rc == 0) rc = launch_combine(static_cast<__half*>(o), lse, ws_o, ws_lse, rows, D, splits, stream);
   cudaFreeAsync(ws, stream);
   return rc;
@@ -408,6 +432,56 @@ int b200_fmha_fwd_f16_seqlens(const void* q, const void* k, const void* v, void*
   const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
   return fmha_run(q, k, v, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
                   static_cast<cudaStream_t>(stream), &lens);
+}
+
+int b200_fmha_fwd_f16_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
+                            const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv,
+                            int Nq, int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
+                            int num_splits, float scale, void* stream) {
+  if (!q || !k_cache || !v_cache || !o || !block_table)
+    return fail(B200_EINVAL, "fmha_paged: null pointer (q, k_cache, v_cache, o and block_table are required)");
+  if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "fmha_paged: bad shape B=%d H=%d D=%d", B, H, D);
+  if (Nq <= 0) return fail(B200_EINVAL, "fmha_paged: bad length Nq=%d (must be >= 1)", Nq);
+  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_paged: causal must be 0 or 1, got %d", causal);
+  if (Hkv <= 0 || H % Hkv != 0)
+    return fail(B200_EINVAL, "fmha_paged: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
+  if (num_splits < 0 || num_splits > kMaxSplits)
+    return fail(B200_EINVAL, "fmha_paged: num_splits=%d must be in 0 .. %d", num_splits, kMaxSplits);
+  if (static_cast<long long>(B) * Hkv > 65535)
+    return fail(B200_EINVAL, "fmha_paged: B*Hkv = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
+  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
+    return fail(B200_EINVAL,
+                "fmha_paged: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)");
+  if (static_cast<long long>(H / Hkv) * Nq > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "fmha_paged: (H/Hkv)*Nq = %lld query rows per K/V head exceed 2^31 - 1",
+                static_cast<long long>(H / Hkv) * Nq);
+  if ((reinterpret_cast<uintptr_t>(seqlens_q) & 3u) != 0)
+    return fail(B200_EINVAL, "fmha_paged: seqlens_q must be 4-byte aligned (int32)");
+  if ((reinterpret_cast<uintptr_t>(seqlens_k) & 3u) != 0)
+    return fail(B200_EINVAL, "fmha_paged: seqlens_k must be 4-byte aligned (int32)");
+  if ((reinterpret_cast<uintptr_t>(block_table) & 3u) != 0)
+    return fail(B200_EINVAL, "fmha_paged: block_table must be 4-byte aligned (int32)");
+  if (num_pages < 1) return fail(B200_EINVAL, "fmha_paged: num_pages=%d must be >= 1", num_pages);
+  if (max_pages_per_seq < 1)
+    return fail(B200_EINVAL, "fmha_paged: max_pages_per_seq=%d must be >= 1", max_pages_per_seq);
+  if (page_size < 16 || (page_size & (page_size - 1)) != 0)
+    return fail(B200_EINVAL, "fmha_paged: page_size=%d must be a power of two >= 16", page_size);
+  if (static_cast<long long>(num_pages) * page_size > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "fmha_paged: num_pages*page_size = %lld pool rows exceed 2^31 - 1",
+                static_cast<long long>(num_pages) * page_size);
+  if (static_cast<long long>(max_pages_per_seq) * page_size > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "fmha_paged: max_pages_per_seq*page_size = %lld keys per sequence exceed 2^31 - 1",
+                static_cast<long long>(max_pages_per_seq) * page_size);
+  if (D % 8 != 0) return fail(B200_ENOTSUP, "fmha_paged: headdim not support! (D=%d must be a multiple of 8)", D);
+  if (D > 1024) return fail(B200_ENOTSUP, "fmha_paged: headdim not support! (D=%d > 1024)", D);
+  if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
+  const int G = H / Hkv, Nk = max_pages_per_seq * page_size;
+  // everything but the K/V addressing is b200_fmha_fwd_f16_seqlens on the padded Nk, the split count included
+  const int splits = num_splits == 0 ? auto_splits(B, Hkv, G, Nq, Nk, D) : num_splits;
+  const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
+  const attn::Pages pages{block_table, page_size, max_pages_per_seq};
+  return fmha_run(q, k_cache, v_cache, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
+                  static_cast<cudaStream_t>(stream), &lens, &pages, num_pages);
 }
 
 int b200_fmha_fwd_f16_rmsnorm(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H,

@@ -45,6 +45,19 @@
 //   * keys >= Lk_b are masked like the tail past Nk; V rows >= Lk_b of the one partial key block are zeroed in shared
 //     memory (producer warp 1) before the consumers read them, since P = 0 times a NaN or Inf of V is NaN;
 //   * padded rows and rows without a visible key store O = 0 and lse = -inf as literal values.
+//
+// Paged K/V (attn_fwd_paged_kernel, b200_fmha_fwd_f16_paged): K and V are pools [num_pages, page_size, Hkv, D] and
+// sequence b's key t is row t % page_size of page table[b][t / page_size]; everything else is the per-sequence-length
+// kernel with the padded Nk = max_pages * page_size.
+//   * the K / V tensor maps are {D, Hkv, num_pages * page_size} with a box {64, 1, R}, R = min(page_size, kBN): a
+//     {64 d, kBN keys} chunk is kBN / R sub-loads into one ring slot, sub-load i at slot + i * R * 128 bytes (a multiple
+//     of 1024, so the 128B swizzle is that of one kBN-row box), all onto the slot's full barrier with the usual tx count;
+//   * the producer is a whole warp: lane i holds the pool row of sub-load i of the next key block, read one block ahead
+//     (the table load's latency hides behind the current block's issues) and broadcast to lane 0 with __shfl_sync;
+//   * sub-loads past the sequence's last page, ceil(Lk_b / page_size) - 1, read that page again instead of the table:
+//     their keys are masked and their V rows zeroed, since the partial key block's V rows past Lk_b come from real pages
+//     (zeroed whenever Lk_b % kBN != 0, not only below the padded Nk);
+//   * a page id is only a TMA coordinate: one outside [0, num_pages) reads zeros (wrong values, no out-of-bounds access).
 #pragma once
 #include <cuda.h>
 
@@ -78,6 +91,13 @@ struct Lens {
   const int* q;
   const int* k;
   int hkv;
+};
+
+// attn_fwd_paged_kernel: the block table (int32 [B, max_pages] on the device) and the page size (a power of two >= 16)
+struct Pages {
+  const int* table;
+  int page_size;
+  int max_pages;
 };
 
 // Keys whose exponential the D <= 128 kernels evaluate on the FMA pipe (exp2_fma_pipe) instead of MUFU.EX2: bit i
@@ -156,13 +176,15 @@ __device__ __forceinline__ int2 kv_blocks(const Params& p, int q0, int row_end, 
 
 // kDS: columns of O per CTA (64, 128 or 256); kBN: keys per block; kVT: V is [B,H,D,N]; kCausal: the causal mask;
 // kGQA: the causal mask on packed query heads; kSplit: split-KV; kSeqlens: per-sequence lengths from `lens` (see the top
-// of this file).  kCausal, kGQA, kSplit and kSeqlens are template parameters so that the other kernels compile to the
-// code they had without them.
-template <int kDS, int kBN, int kWG, bool kVT, bool kCausal, bool kGQA, bool kSplit, bool kSeqlens>
+// of this file); kPaged: K and V in pages of a pool through `pages` (implies kSeqlens).  kCausal, kGQA, kSplit, kSeqlens
+// and kPaged are template parameters so that the other kernels compile to the code they had without them.
+template <int kDS, int kBN, int kWG, bool kVT, bool kCausal, bool kGQA, bool kSplit, bool kSeqlens, bool kPaged = false>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k,
-                                              const CUtensorMap& tmap_v, Params p, const Lens& lens) {
+                                              const CUtensorMap& tmap_v, Params p, const Lens& lens,
+                                              const Pages& pages = Pages{}) {
   static_assert(!kVT || kDS <= 128, "transposed V: one slab of <= 128 columns");
   static_assert(!kSeqlens || (!kVT && kGQA), "per-sequence lengths: natural V, query positions of packed rows");
+  static_assert(!kPaged || kSeqlens, "paged K/V: per-sequence lengths");
   constexpr int SLOT = slot_bytes(kBN, kDS, kVT);
   constexpr int KV_BYTES = 64 * kBN * 2;   // one {64 columns, kBN keys} chunk of K or V
   constexpr int NS = kBN / 2;     // S accumulator registers per thread
@@ -213,11 +235,12 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
   // V chunks of this slab per key block
   const int nvc = kVT ? kBN / 64 : min(NDC, (p.D - d0 + 63) / 64);
   // kSeqlens: the visited key block that ends past Lk_b inside the K/V buffers (-1: none).  TMA zero-fills only past
-  // nk_pad, so its V rows of keys >= Lk_b are zeroed in shared memory before the consumers read them.
+  // nk_pad, so its V rows of keys >= Lk_b are zeroed in shared memory before the consumers read them.  kPaged: every
+  // row of a sub-load comes from a page, so any partial key block is one.
   [[maybe_unused]] int vz = -1;
   [[maybe_unused]] const uint32_t vbar = rowss;   // its V chunks land here (no fused RMS norm with kSeqlens)
   if constexpr (kSeqlens) {
-    if (p.Nk % kBN != 0 && p.Nk < nk_pad && p.num_kv - 1 >= kv.x && p.num_kv - 1 < kv.y) vz = p.num_kv - 1;
+    if (p.Nk % kBN != 0 && (kPaged || p.Nk < nk_pad) && p.num_kv - 1 >= kv.x && p.num_kv - 1 < kv.y) vz = p.num_kv - 1;
   }
 
   if (threadIdx.x == 0) {
@@ -233,7 +256,54 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
 
   if (wg == 0) {
     if constexpr (kWG > 1) reg_dealloc<40>();
-    if (tid == 0) {
+    if constexpr (kPaged) {
+      if (tid < 32) {
+        // lane 0 issues; lane i < nsub holds the pool row of sub-load i of a key block (the top of this file)
+        const int lane = tid, ps = pages.page_size, shift = __ffs(ps) - 1;
+        const int R = min(ps, kBN), nsub = kBN / R;
+        const int hk = blockIdx.y % lens.hkv;
+        const int* table = pages.table + static_cast<size_t>(blockIdx.y / lens.hkv) * pages.max_pages;
+        const int last = ((p.Nk + ps - 1) >> shift) - 1;   // the sequence's last page (p.Nk >= 1 if a block is visited)
+        auto pool_row = [&](int j) {
+          const int t = j * kBN + min(lane, nsub - 1) * R;
+          const unsigned page = static_cast<unsigned>(__ldg(table + min(t >> shift, last)));
+          return static_cast<int>((page << shift) + static_cast<unsigned>(t & (ps - 1)));
+        };
+        if (lane == 0) {
+          prefetch_tmap(&tmap_q);
+          prefetch_tmap(&tmap_k);
+          prefetch_tmap(&tmap_v);
+          mbar_expect_tx(qbar, kWG * p.nq * 8192);
+          for (int w = 0; w < kWG; ++w)
+            for (int c = 0; c < p.nq; ++c)
+              tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, q0 + 64 * w, bh, kEvictFirst);
+        }
+        int it = 0;
+        int row = kv.x < kv.y ? pool_row(kv.x) : 0;
+        for (int j = kv.x; j < kv.y; ++j) {
+          const int cur = row;
+          if (j + 1 < kv.y) row = pool_row(j + 1);   // one block ahead
+          // the block's K chunks, then its V chunks; the partial block's V onto vbar, as below
+          for (int c = 0; c < p.nq + nvc; ++c, ++it) {
+            const bool isv = c >= p.nq, zeroed = isv && j == vz;
+            const int s = it % p.ring;
+            const uint32_t bar = zeroed ? vbar : full(s);
+            if (lane == 0) {
+              if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
+              if (!zeroed) mbar_expect_tx(bar, KV_BYTES);
+              else if (c == p.nq) mbar_expect_tx(vbar, nvc * KV_BYTES);
+            }
+            for (int i = 0; i < nsub; ++i) {
+              const int r = __shfl_sync(0xffffffffu, cur, i);
+              if (lane == 0)
+                tma_load_3d(sring + s * SLOT + i * R * 128, isv ? &tmap_v : &tmap_k, bar,
+                            isv ? d0 + 64 * (c - p.nq) : 64 * c, hk, r, kEvictLast);
+            }
+          }
+        }
+      }
+    }
+    if (!kPaged && tid == 0) {
       prefetch_tmap(&tmap_q);
       prefetch_tmap(&tmap_k);
       prefetch_tmap(&tmap_v);
@@ -573,6 +643,14 @@ __global__ void __launch_bounds__(threads<kWG>(), 1)
 attn_fwd_seqlens_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                         const __grid_constant__ CUtensorMap tmap_v, const Params p, const Lens lens) {
   attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, kSplit, true>(tmap_q, tmap_k, tmap_v, p, lens);
+}
+
+// Paged K/V (b200_fmha_fwd_f16_paged): the per-sequence-length kernel reading K and V through a block table.
+template <int kDS, int kBN, int kWG, bool kCausal, bool kSplit>
+__global__ void __launch_bounds__(threads<kWG>(), 1)
+attn_fwd_paged_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                      const __grid_constant__ CUtensorMap tmap_v, const Params p, const Lens lens, const Pages pages) {
+  attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, kSplit, true, true>(tmap_q, tmap_k, tmap_v, p, lens, pages);
 }
 
 }  // namespace attn

@@ -100,7 +100,7 @@ def _check(Q, K, V, O, v_transposed):
 
 
 def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=None, causal: bool = False,
-             num_splits: int = 1, seqlens_q=None, seqlens_k=None) -> None:
+             num_splits: int = 1, seqlens_q=None, seqlens_k=None, block_table=None) -> None:
     """``O = softmax(Q K^T * scale) V`` on the current CUDA stream of ``Q``'s device.
 
     Q, O are ``[B,H,Nq,D]``; K is ``[B,Hkv,Nk,D]`` and V ``[B,Hkv,Nk,D]`` (or ``[B,Hkv,D,Nk]`` with ``v_transposed``),
@@ -123,7 +123,19 @@ def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=
     ``0 .. clamp(seqlens_q[b], 0, Nq) - 1`` and key rows ``0 .. clamp(seqlens_k[b], 0, Nk) - 1``; keys past that
     contribute nothing whatever they hold, the causal diagonal is per sequence, and padded query rows get O = 0,
     lse = -inf.  The lengths are read on the GPU only (no host synchronisation), so a captured CUDA graph replays with
-    whatever lengths the tensors hold.  None means Nq resp. Nk for every sequence; natural V only."""
+    whatever lengths the tensors hold.  None means Nq resp. Nk for every sequence; natural V only.
+
+    ``block_table`` (int32 contiguous CUDA tensor ``[B, max_pages_per_seq]`` on Q's device) makes K and V paged KV-cache
+    pools ``[num_pages, page_size, Hkv, D]`` (``b200_fmha_fwd_f16_paged``, the layout of FlashAttention's
+    ``flash_attn_with_kvcache(block_table=...)``): key t of sequence b is row ``t % page_size`` of page
+    ``block_table[b, t // page_size]``.  The call is then the ``seqlens_q`` / ``seqlens_k`` call on a padded cache of
+    ``Nk = max_pages_per_seq * page_size`` keys, bit for bit, without gathering the pages.  Table entries past a
+    sequence's last used page are never read (pad with -1 or stale ids); pages may be shared between sequences.  The
+    table is read on the GPU only, so a captured graph replays with whatever tables and lengths the tensors hold.
+    page_size must be a power of two >= 16; natural V only."""
+    if block_table is not None:
+        _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table)
+        return
     if seqlens_q is not None or seqlens_k is not None:
         _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k)
         return
@@ -142,6 +154,16 @@ def _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seql
         raise RuntimeError("leetcuda_b200.flash_attn: seqlens_q / seqlens_k take natural V [B,Hkv,Nk,D] only "
                            "(v_transposed=True is not supported with lengths)")
     B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, False, same_length=False, grouped=True)
+    _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k)
+    _placement(Q, K, V, O, *(() if lse is None else (lse,)))
+    args = [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), None if lse is None else lse.data_ptr(),
+            None if seqlens_q is None else seqlens_q.data_ptr(), None if seqlens_k is None else seqlens_k.data_ptr(),
+            B, H, Hkv, Nq, Nk, D, int(bool(causal)), int(num_splits), float(scale)]
+    _call_on_device(_capi.lib().b200_fmha_fwd_f16_seqlens, args, Q.device.index)
+
+
+def _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k) -> None:
+    """num_splits, lse and the length arrays of the seqlens and paged calls."""
     if isinstance(num_splits, bool) or not isinstance(num_splits, int) or not 0 <= num_splits <= _capi.FMHA_MAX_SPLITS:
         raise RuntimeError(f"leetcuda_b200.flash_attn: num_splits must be an int in 0 .. {_capi.FMHA_MAX_SPLITS}, "
                            f"got {num_splits!r}")
@@ -154,12 +176,41 @@ def _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seql
                 or not t.is_contiguous() or t.device != Q.device:
             raise RuntimeError(f"leetcuda_b200.flash_attn: {name} must be an int32 contiguous CUDA tensor [B] = [{B}] "
                                f"on Q's device")
+
+
+def _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table) -> None:
+    if v_transposed:
+        raise RuntimeError("leetcuda_b200.flash_attn: block_table takes natural V pools [num_pages,page_size,Hkv,D] "
+                           "only (v_transposed=True is not supported with a block table)")
+    for t in (Q, K, V, O):
+        if t.dtype != torch.float16:
+            raise RuntimeError("values must be torch::kHalf")
+    if Q.dim() != 4 or tuple(O.shape) != tuple(Q.shape):
+        raise RuntimeError("Tensor size mismatch!")
+    B, H, Nq, D = Q.shape
+    if K.dim() != 4 or tuple(K.shape) != tuple(V.shape) or K.shape[3] != D or K.shape[2] < 1 or H % K.shape[2] \
+            or K.shape[0] < 1:
+        raise RuntimeError(f"leetcuda_b200.flash_attn: with block_table, K and V must be pools "
+                           f"[num_pages, page_size, Hkv, D] of the same shape, with D = {D} and Hkv dividing H = {H}")
+    num_pages, page_size, Hkv, _ = K.shape
+    if page_size < 16 or page_size & (page_size - 1):
+        raise RuntimeError(f"leetcuda_b200.flash_attn: page_size (K.shape[1]) must be a power of two >= 16, "
+                           f"got {page_size}")
+    _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k)
+    t = block_table
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or t.dim() != 2 or t.shape[0] != B \
+            or t.shape[1] < 1 or not t.is_cuda or not t.is_contiguous() or t.device != Q.device:
+        raise RuntimeError(f"leetcuda_b200.flash_attn: block_table must be an int32 contiguous CUDA tensor "
+                           f"[B, max_pages_per_seq] = [{B}, >= 1] on Q's device")
     _placement(Q, K, V, O, *(() if lse is None else (lse,)))
-    idx = Q.device.index
     args = [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), None if lse is None else lse.data_ptr(),
-            None if seqlens_q is None else seqlens_q.data_ptr(), None if seqlens_k is None else seqlens_k.data_ptr(),
-            B, H, Hkv, Nq, Nk, D, int(bool(causal)), int(num_splits), float(scale)]
-    fn = _capi.lib().b200_fmha_fwd_f16_seqlens
+            t.data_ptr(), None if seqlens_q is None else seqlens_q.data_ptr(),
+            None if seqlens_k is None else seqlens_k.data_ptr(), B, H, Hkv, Nq, num_pages, page_size, t.shape[1], D,
+            int(bool(causal)), int(num_splits), float(scale)]
+    _call_on_device(_capi.lib().b200_fmha_fwd_f16_paged, args, Q.device.index)
+
+
+def _call_on_device(fn, args, idx) -> None:
     if torch.cuda.current_device() != idx:
         with torch.cuda.device(idx):
             rc = fn(*args, _capi.raw_stream(idx))

@@ -10,19 +10,47 @@ namespace {
 using namespace b200;
 using b200::host::fail;
 
+// Persistent launch in clusters of `cs` CTAs (1 or 2; p.num_tiles counts cluster tiles).  A cluster of two occupies two
+// SMs of one GPC, so with cs = 2 the grid is as many clusters as fit the GPU at once (cached per device), not #SMs / 2:
+// a GPC with an odd number of SMs then leaves one SM idle instead of running a cluster in a second wave.
 template <int kBN, bool kBMn, bool kTf32, bool kAcc16>
-int launch_hgemm(const CUtensorMap& ta, const CUtensorMap& tb, const hgemm::Params& p, int grid, cudaStream_t stream) {
+int launch_hgemm(const CUtensorMap& ta, const CUtensorMap& tb, const hgemm::Params& p, int cs, cudaStream_t stream) {
   using C_ = hgemm::Cfg<kBN>;
   auto kern = hgemm::hgemm_wgmma_kernel<kBN, kBMn, kTf32, kAcc16>;
   static bool attr_set[64] = {false};
+  static int max_clusters[64] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
+  const bool cached = dev >= 0 && dev < 64;
+  if (!cached || !attr_set[dev]) {
     B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES));
-    attr_set[dev] = true;
+    if (cached) attr_set[dev] = true;
   }
-  kern<<<grid, hgemm::kThreads, C_::SMEM_BYTES, stream>>>(ta, tb, p);
-  B200_CUDA_OK(cudaGetLastError());
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.blockDim = dim3(hgemm::kThreads, 1, 1);
+  cfg.dynamicSmemBytes = C_::SMEM_BYTES;
+  cfg.stream = stream;
+  cudaLaunchAttribute attrs[1];
+  attrs[0].id = cudaLaunchAttributeClusterDimension;
+  attrs[0].val.clusterDim.x = static_cast<unsigned>(cs);
+  attrs[0].val.clusterDim.y = 1;
+  attrs[0].val.clusterDim.z = 1;
+  cfg.attrs = attrs;
+  cfg.numAttrs = 1;
+  int slots = host::sm_count();
+  if (cs > 1) {
+    slots = cached ? max_clusters[dev] : 0;
+    if (slots == 0) {
+      cfg.gridDim = dim3(static_cast<unsigned>(cs), 1, 1);
+      B200_CUDA_OK(cudaOccupancyMaxActiveClusters(&slots, kern, &cfg));
+      if (slots <= 0) return fail(B200_ECUDA, "hgemm: no cluster of %d CTAs fits the device", cs);
+      if (cached) max_clusters[dev] = slots;
+    }
+  }
+  const int grid = cs * (p.num_tiles < slots ? p.num_tiles : slots);
+  cfg.gridDim = dim3(static_cast<unsigned>(grid), 1, 1);
+  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, ta, tb, p));
   host::count_launch();
   return 0;
 }
@@ -141,11 +169,18 @@ int hgemm_impl(const void* a, const void* b, void* c, int M, int N, int K, int b
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int sms = host::sm_count();
 
+  // Clusters of two CTAs share each B tile (see hgemm_sm90.cuh) whenever there are two m-tiles to pair.
+  const int tiles_m = (M + hgemm::BM - 1) / hgemm::BM;
+  const int cs = tiles_m >= 2 ? 2 : 1;
+
   // Tile: 128x256 (least operand traffic per flop) unless a 128x128 tiling fills the last wave of the
-  // SMs markedly better (mid-size problems would otherwise leave many of the SMs idle).
+  // SMs markedly better (mid-size problems would otherwise leave many of the SMs idle).  With an odd tiles_m the
+  // last cluster row's second m-tile lies past M and still takes an SM: it counts towards the waves, not the work.
   auto score = [&](int bnc, double eff) {
-    const long tiles = static_cast<long>((M + 127) / 128) * ((N + bnc - 1) / bnc);
-    const long waves = (tiles + sms - 1) / sms;
+    const long tn = (N + bnc - 1) / bnc;
+    const long tiles = static_cast<long>(tiles_m) * tn;
+    const long launched = static_cast<long>((tiles_m + cs - 1) / cs * cs) * tn;
+    const long waves = (launched + sms - 1) / sms;
     return eff * static_cast<double>(tiles) / static_cast<double>(waves * sms);
   };
   const int bn = score(128, 0.90) > score(256, 1.0) ? 128 : 256;
@@ -154,9 +189,9 @@ int hgemm_impl(const void* a, const void* b, void* c, int M, int N, int K, int b
   memset(&p, 0, sizeof(p));
   p.C = c;
   p.M = M; p.N = N; p.K = K; p.ldc = N;
-  p.tiles_m = (M + hgemm::BM - 1) / hgemm::BM;
+  p.tiles_m = tiles_m;
   p.tiles_n = (N + bn - 1) / bn;
-  p.num_tiles = p.tiles_m * p.tiles_n;
+  p.num_tiles = (tiles_m + cs - 1) / cs * p.tiles_n;
   if (fan) {
     if (fan->n_peers < 0 || fan->n_peers > 7) return fail(B200_EINVAL, "hgemm: %d peers", fan->n_peers);
     if (fan->mc) p.C_mc = static_cast<char*>(fan->mc) + fan->elem_offset * esize;
@@ -178,7 +213,7 @@ int hgemm_impl(const void* a, const void* b, void* c, int M, int N, int K, int b
   if (b_layout == B200_B_ROW_MAJOR_NK) {
     uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(N)};
     uint64_t str[1] = {static_cast<uint64_t>(K) * esize};
-    uint32_t box[2] = {static_cast<uint32_t>(bke), static_cast<uint32_t>(bn)};
+    uint32_t box[2] = {static_cast<uint32_t>(bke), static_cast<uint32_t>(bn / cs)};   // each CTA loads 1/cs of B
     int rc = host::get_tmap(&tb, b, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, dt);
     if (rc) return rc;
   } else {
@@ -189,24 +224,22 @@ int hgemm_impl(const void* a, const void* b, void* c, int M, int N, int K, int b
     if (rc) return rc;
   }
 
-  const int grid = p.num_tiles < sms ? p.num_tiles : sms;
-
   const bool mn = (b_layout == B200_B_ROW_MAJOR_KN);
   if (tf32)
-    return bn == 128 ? launch_hgemm<128, false, true, false>(ta, tb, p, grid, stream)
-                     : launch_hgemm<256, false, true, false>(ta, tb, p, grid, stream);
+    return bn == 128 ? launch_hgemm<128, false, true, false>(ta, tb, p, cs, stream)
+                     : launch_hgemm<256, false, true, false>(ta, tb, p, cs, stream);
   if (acc_f16) {
     if (bn == 128)
-      return mn ? launch_hgemm<128, true, false, true>(ta, tb, p, grid, stream)
-                : launch_hgemm<128, false, false, true>(ta, tb, p, grid, stream);
-    return mn ? launch_hgemm<256, true, false, true>(ta, tb, p, grid, stream)
-              : launch_hgemm<256, false, false, true>(ta, tb, p, grid, stream);
+      return mn ? launch_hgemm<128, true, false, true>(ta, tb, p, cs, stream)
+                : launch_hgemm<128, false, false, true>(ta, tb, p, cs, stream);
+    return mn ? launch_hgemm<256, true, false, true>(ta, tb, p, cs, stream)
+              : launch_hgemm<256, false, false, true>(ta, tb, p, cs, stream);
   }
   if (bn == 128)
-    return mn ? launch_hgemm<128, true, false, false>(ta, tb, p, grid, stream)
-              : launch_hgemm<128, false, false, false>(ta, tb, p, grid, stream);
-  return mn ? launch_hgemm<256, true, false, false>(ta, tb, p, grid, stream)
-            : launch_hgemm<256, false, false, false>(ta, tb, p, grid, stream);
+    return mn ? launch_hgemm<128, true, false, false>(ta, tb, p, cs, stream)
+              : launch_hgemm<128, false, false, false>(ta, tb, p, cs, stream);
+  return mn ? launch_hgemm<256, true, false, false>(ta, tb, p, cs, stream)
+            : launch_hgemm<256, false, false, false>(ta, tb, p, cs, stream);
 }
 
 // cached device workspace for the *_host wrappers (per thread and device).  Those entry points return only after their

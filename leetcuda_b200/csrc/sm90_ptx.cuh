@@ -29,6 +29,17 @@ B200_DEVICE void cluster_sync_all() {
   cluster_arrive();
   cluster_wait();
 }
+// rank of this CTA in its cluster, and the number of CTAs in the cluster (1 for a launch without clusters)
+B200_DEVICE uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+B200_DEVICE uint32_t cluster_nctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+  return r;
+}
 template <int N>
 B200_DEVICE void reg_dealloc() {
   asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
@@ -58,6 +69,12 @@ B200_DEVICE void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 }
 B200_DEVICE void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// arrive on an mbarrier of another CTA of the cluster; `bar` is a shared::cluster address (see mapa).  The default
+// .release.cta semantics: .release.cluster compiles to a MEMBAR.ALL.GPU before the arrive, which in a wgmma loop
+// waits for every global store the thread still has in flight.
+B200_DEVICE void mbar_arrive_cluster(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 B200_DEVICE bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
@@ -108,6 +125,16 @@ B200_DEVICE void tma_load_2d(uint32_t dst, const void* tmap, uint32_t bar, int c
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
       " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst),
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "l"(hint)
+      : "memory");
+}
+// the same box into the shared memory of every CTA of the cluster whose bit is set in `cta_mask`, at offset `dst` of
+// each; every one of them gets the complete_tx on its own mbarrier at offset `bar`
+B200_DEVICE void tma_load_2d_multicast(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, uint16_t cta_mask,
+                                       uint64_t hint = kEvictNormal) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask), "l"(hint)
       : "memory");
 }
 B200_DEVICE void tma_load_3d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2,

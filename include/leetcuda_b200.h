@@ -213,6 +213,25 @@ int b200_fmha_fwd_f16_paged(const void* q, const void* k_cache, const void* v_ca
                             int H, int Hkv, int Nq, int num_pages, int page_size, int max_pages_per_seq, int D,
                             int causal, int num_splits, float scale, void* stream);
 
+/* bf16 attention: b200_fmha_fwd_f16_seqlens and b200_fmha_fwd_f16_paged with q, k, v (k_cache, v_cache) and o in
+ * bf16.  Argument lists, constraints, error codes and messages, and semantics are those of the f16 entries: the length
+ * clamps, the per-sequence bottom-right causal mask, O = 0 and lse = -inf in padded rows and rows without a key, the
+ * GQA mapping, num_splits (0 chooses b200_fmha_fwd_f16_gqa_splits(B, H, Hkv, Nq, Nk, D), which does not depend on
+ * the element type), the split workspace and its combine, and the lengths and tables read on the GPU only.  lse stays
+ * fp32.  NULL seqlens_q and seqlens_k give the dense call (one length Nq / Nk for every sequence, MHA or GQA, causal
+ * or not, split or not).  The element type is the only difference: S and O accumulate in fp32 as for fp16, P is
+ * rounded to bf16 (nearest even) before P V, and O is rounded once to bf16.  bf16 has fp32's exponent range, so
+ * inputs and outputs beyond fp16's 65504 are fine.  Natural V only, as for the f16 entries. */
+int b200_fmha_fwd_bf16_seqlens(const void* q, const void* k, const void* v, void* o, float* lse /* may be NULL */,
+                               const int* seqlens_q /* may be NULL */, const int* seqlens_k /* may be NULL */,
+                               int B, int H, int Hkv, int Nq, int Nk, int D, int causal, int num_splits, float scale,
+                               void* stream);
+int b200_fmha_fwd_bf16_paged(const void* q, const void* k_cache, const void* v_cache, void* o,
+                             float* lse /* may be NULL */, const int* block_table,
+                             const int* seqlens_q /* may be NULL */, const int* seqlens_k /* may be NULL */, int B,
+                             int H, int Hkv, int Nq, int num_pages, int page_size, int max_pages_per_seq, int D,
+                             int causal, int num_splits, float scale, void* stream);
+
 /* ------------------------------------------------------------------ SGEMM (TF32)
  * C[M,N] (fp32) = A[M,K] (fp32) x B on the tensor cores through wgmma .tf32 with fp32
  * accumulation — the sibling of the HGEMM path (SURVEY §8f-2).  Replaces

@@ -6,12 +6,14 @@
 
 #include <algorithm>
 
-#include "capi_common.cuh"
-#include "attn_sm90.cuh"
+#include <type_traits>
+
+#include "attn_launch.cuh"
 
 namespace {
 
 using namespace b200;
+using b200::attn::launch_kernel;
 using b200::host::fail;
 
 // Split-KV: the most splits b200_fmha_fwd_f16_gqa accepts (B200_FMHA_MAX_SPLITS); for num_splits = 0 the fewest key
@@ -23,35 +25,6 @@ using b200::host::fail;
 constexpr int kMaxSplits = 64;
 constexpr int kMinBlocksPerSplit = 4;
 constexpr int kMinBlocksToSplit = 16;
-
-// One attention kernel on a grid of (query tiles x slabs, K/V heads, splits); attr_smem[dev] remembers the dynamic
-// shared memory the kernel was allowed on each device.
-template <typename... Params, typename... Args>
-int launch_kernel(void (*kern)(Params...), int* attr_smem, const attn::Params& p, int qtiles, int BH, int splits,
-                  int threads, int smem, cudaStream_t stream, const Args&... args) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && attr_smem[dev] < smem) {
-    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_smem[dev] = smem;
-  }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(static_cast<unsigned>(qtiles * p.slabs), static_cast<unsigned>(BH), static_cast<unsigned>(splits));
-  cfg.blockDim = dim3(threads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeClusterDimension;   // the slabs of one query tile (fused RMS norm)
-  attrs[0].val.clusterDim.x = (p.rms_g > 0.f) ? static_cast<unsigned>(p.slabs) : 1u;
-  attrs[0].val.clusterDim.y = 1;
-  attrs[0].val.clusterDim.z = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = 1;
-  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, args...));
-  host::count_launch();
-  return 0;
-}
 
 // lens != nullptr: per-sequence lengths, attn_fwd_seqlens_kernel (natural V only); with pages also: paged K/V,
 // attn_fwd_paged_kernel
@@ -110,14 +83,19 @@ __global__ void transpose_dn_to_nd_kernel(const __half* __restrict__ in, __half*
 }
 
 // out[r, :] = sum_s w_s o_s[r, :] / sum_s w_s,  w_s = exp(lse_s[r] - max_s lse_s[r]),  out_lse[r] = ln sum_s w_s + max
-// over the fp32 parts the split kernel wrote (ws_o [splits, rows, D], ws_lse [splits, rows]), rounded once to fp16.  A
+// over the fp32 parts the split kernel wrote (ws_o [splits, rows, D], ws_lse [splits, rows]), rounded once to T.  A
 // row whose parts are all empty (lse -inf) gets 0 and -inf: the max is clamped to -FLT_MAX, every weight is 0, and the
 // divisor is clamped to 1 (otherwise one weight is expf(0) = 1, so the clamp changes nothing).
-// HBM-bound: one thread per 16-byte pack of the output (8 halves), 32 bytes and one lse read per split.
-template <typename Idx>
+// HBM-bound: one thread per 16-byte pack of the output (8 elements), 32 bytes and one lse read per split.  T: __half or
+// __nv_bfloat16.
+template <typename Idx, typename T = __half>
 __global__ void __launch_bounds__(256)
-attn_combine_kernel(__half* __restrict__ out, float* __restrict__ out_lse, const float* __restrict__ ws_o,
+attn_combine_kernel(T* __restrict__ out, float* __restrict__ out_lse, const float* __restrict__ ws_o,
                     const float* __restrict__ ws_lse, unsigned rows, unsigned packs_per_row, int splits) {
+  auto pack = [](float lo, float hi) {
+    if constexpr (std::is_same_v<T, __nv_bfloat16>) return pack_bf162(lo, hi);
+    else return pack_half2(lo, hi);
+  };
   const Idx n_packs = static_cast<Idx>(rows) * packs_per_row;
   const Idx pk = static_cast<Idx>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (pk >= n_packs) return;
@@ -139,15 +117,16 @@ attn_combine_kernel(__half* __restrict__ out, float* __restrict__ out_lse, const
   }
   const float inv = 1.f / fmaxf(denom, 1.f);
   uint4 r;
-  r.x = pack_half2(acc[0] * inv, acc[1] * inv);
-  r.y = pack_half2(acc[2] * inv, acc[3] * inv);
-  r.z = pack_half2(acc[4] * inv, acc[5] * inv);
-  r.w = pack_half2(acc[6] * inv, acc[7] * inv);
+  r.x = pack(acc[0] * inv, acc[1] * inv);
+  r.y = pack(acc[2] * inv, acc[3] * inv);
+  r.z = pack(acc[4] * inv, acc[5] * inv);
+  r.w = pack(acc[6] * inv, acc[7] * inv);
   st_stream(reinterpret_cast<uint4*>(out) + pk, r);
   if (out_lse != nullptr && pk == row * packs_per_row) out_lse[row] = logf(denom) + top;   // first pack of the row
 }
 
-int launch_combine(__half* out, float* out_lse, const float* ws_o, const float* ws_lse, size_t rows, int D, int splits,
+template <typename T>
+int launch_combine(T* out, float* out_lse, const float* ws_o, const float* ws_lse, size_t rows, int D, int splits,
                    cudaStream_t stream) {
   const unsigned ppr = static_cast<unsigned>(D / 8);
   const size_t total = rows * ppr;
@@ -155,9 +134,9 @@ int launch_combine(__half* out, float* out_lse, const float* ws_o, const float* 
   if (rows > 0xFFFFFFFFull || blocks > 0x7FFFFFFFull) return fail(B200_EINVAL, "fmha_gqa: too many output rows");
   const unsigned g = static_cast<unsigned>(blocks), nr = static_cast<unsigned>(rows);
   if (total + 256 < 0xFFFFFFFFull)
-    attn_combine_kernel<unsigned><<<g, 256, 0, stream>>>(out, out_lse, ws_o, ws_lse, nr, ppr, splits);
+    attn_combine_kernel<unsigned, T><<<g, 256, 0, stream>>>(out, out_lse, ws_o, ws_lse, nr, ppr, splits);
   else
-    attn_combine_kernel<size_t><<<g, 256, 0, stream>>>(out, out_lse, ws_o, ws_lse, nr, ppr, splits);
+    attn_combine_kernel<size_t, T><<<g, 256, 0, stream>>>(out, out_lse, ws_o, ws_lse, nr, ppr, splits);
   B200_CUDA_OK(cudaGetLastError());
   host::count_launch();
   return 0;
@@ -180,6 +159,8 @@ Family family(int D) {
 // G: query heads per K/V head (H = G * Hkv; the kernel sees B * Hkv heads of G * Nq packed rows).  splits > 1: grid.z
 // splits whose fp32 parts go to ws_o / ws_lse instead of o / lse (kSplit kernels).  Causal with G > 1 runs kGQA.
 // pages: k and v are pools of num_pages pages [page_size, Hkv, D], and Nk is the padded max_pages * page_size.
+// T: the element type of q, k, v and o; __nv_bfloat16 runs the bf16 kernels (attn_bf16.cu), which take lens always.
+template <typename T>
 int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int Hkv, int G,
                   int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, float* ws_o, float* ws_lse,
                   cudaStream_t stream, const attn::Lens* lens = nullptr, const attn::Pages* pages = nullptr,
@@ -217,6 +198,8 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
   p.tph = causal && Nq >= 64 * wgs ? (Nq + 64 * wgs - 1) / (64 * wgs) : 0;
   const int qtiles = p.tph > 0 ? G * p.tph : (rows + 64 * wgs - 1) / (64 * wgs);
 
+  constexpr bool bf16 = std::is_same_v<T, __nv_bfloat16>;
+  const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUtensorMap tq, tk, tv;
   uint64_t qdims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(rows), BH};
   uint64_t qstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(rows) * D * 2};
@@ -225,30 +208,36 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
   uint32_t qbox[3] = {64, 64, 1};
   uint32_t kbox[3] = {64, static_cast<uint32_t>(bn), 1};
   int rc;
-  if ((rc = host::get_tmap(&tq, q, 3, qdims, qstr, qbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = host::get_tmap(&tq, q, 3, qdims, qstr, qbox, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
   if (pages) {
     // pool rows {D, Hkv, num_pages * page_size}; a key block is kBN / R boxes of R = min(page_size, kBN) rows
     uint64_t pd[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(Hkv),
                       static_cast<uint64_t>(num_pages) * static_cast<uint64_t>(pages->page_size)};
     uint64_t pstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(Hkv) * D * 2};
     uint32_t pbox[3] = {64, 1, static_cast<uint32_t>(std::min(pages->page_size, bn))};
-    if ((rc = host::get_tmap(&tk, k, 3, pd, pstr, pbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-    if ((rc = host::get_tmap(&tv, v, 3, pd, pstr, pbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    if ((rc = host::get_tmap(&tk, k, 3, pd, pstr, pbox, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
+    if ((rc = host::get_tmap(&tv, v, 3, pd, pstr, pbox, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
   } else {
-    if ((rc = host::get_tmap(&tk, k, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    if ((rc = host::get_tmap(&tk, k, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
     if (vt) {
       uint64_t vd[3] = {static_cast<uint64_t>(Nk), static_cast<uint64_t>(D), BH};
       uint64_t vs[2] = {static_cast<uint64_t>(Nk) * 2, static_cast<uint64_t>(Nk) * D * 2};
       uint32_t vb[3] = {64, static_cast<uint32_t>(ds), 1};
-      if ((rc = host::get_tmap(&tv, v, 3, vd, vs, vb, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+      if ((rc = host::get_tmap(&tv, v, 3, vd, vs, vb, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
     } else {
-      if ((rc = host::get_tmap(&tv, v, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+      if ((rc = host::get_tmap(&tv, v, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
     }
   }
   const int bh = static_cast<int>(BH);
   if (vt && lens) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with lengths)");
   const bool pk = G > 1;
   const attn::Pages* pg = pages;
+  if constexpr (bf16) {
+    if (vt || !lens) return fail(B200_EINVAL, "fmha: internal dispatch error (bf16 without lengths or with V^T)");
+    if (ds == 64) return attn::launch_attn_bf16<64, 128, 2>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, stream);
+    if (ds == 128) return attn::launch_attn_bf16<128, 64, 2>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, stream);
+    return attn::launch_attn_bf16<256, 64, 1>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, stream);
+  }
   if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream)
                           : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream);
   if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream)
@@ -258,11 +247,12 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
 }
 
 // The attention kernel, and with splits > 1 its fp32 parts in a stream-ordered workspace and the combine kernel.
+template <typename T>
 int fmha_run(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int Hkv, int G,
              int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, cudaStream_t stream,
              const attn::Lens* lens = nullptr, const attn::Pages* pages = nullptr, int num_pages = 0) {
   if (splits <= 1)
-    return fmha_dispatch(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, 1, nullptr, nullptr, stream,
+    return fmha_dispatch<T>(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, 1, nullptr, nullptr, stream,
                          lens, pages, num_pages);
   const size_t rows = static_cast<size_t>(B) * Hkv * G * Nq;
   const size_t lse_bytes = (static_cast<size_t>(splits) * rows * 4 + 255) & ~static_cast<size_t>(255);
@@ -270,9 +260,9 @@ int fmha_run(const void* q, const void* k, const void* v, void* o, float* lse, f
   B200_CUDA_OK(cudaMallocAsync(&ws, lse_bytes + static_cast<size_t>(splits) * rows * D * 4, stream));
   float* ws_lse = static_cast<float*>(ws);
   float* ws_o = reinterpret_cast<float*>(static_cast<char*>(ws) + lse_bytes);
-  int rc = fmha_dispatch(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, splits, ws_o, ws_lse, stream,
+  int rc = fmha_dispatch<T>(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, splits, ws_o, ws_lse, stream,
                          lens, pages, num_pages);
-  if (rc == 0) rc = launch_combine(static_cast<__half*>(o), lse, ws_o, ws_lse, rows, D, splits, stream);
+  if (rc == 0) rc = launch_combine(static_cast<T*>(o), lse, ws_o, ws_lse, rows, D, splits, stream);
   cudaFreeAsync(ws, stream);
   return rc;
 }
@@ -336,13 +326,102 @@ int fmha_impl(const void* q, const void* k, const void* v, void* o, float* lse, 
       if (le != cudaSuccess) rc = fail(B200_ECUDA, "transpose launch failed: %s", cudaGetErrorString(le));
       else {
         host::count_launch();
-        rc = fmha_run(q, k, ws, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, false, causal, scale, splits, stream);
+        rc = fmha_run<__half>(q, k, ws, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, false, causal, scale, splits, stream);
       }
       cudaFreeAsync(ws, stream);
       return rc;
     }
   }
-  return fmha_run(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, v_transposed != 0, causal, scale, splits, stream);
+  return fmha_run<__half>(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, v_transposed != 0, causal, scale, splits, stream);
+}
+
+// b200_fmha_fwd_{f16,bf16}_seqlens and _paged: the same checks and messages for both element types T.
+template <typename T>
+int fmha_seqlens(const void* q, const void* k, const void* v, void* o, float* lse, const int* seqlens_q,
+                              const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk, int D, int causal,
+                              int num_splits, float scale, void* stream) {
+  if (!q || !k || !v || !o) return fail(B200_EINVAL, "fmha_seqlens: null pointer (q, k, v and o are required)");
+  if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "fmha_seqlens: bad shape B=%d H=%d D=%d", B, H, D);
+  if (Nq <= 0 || Nk <= 0)
+    return fail(B200_EINVAL, "fmha_seqlens: bad lengths Nq=%d Nk=%d (both must be >= 1)", Nq, Nk);
+  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_seqlens: causal must be 0 or 1, got %d", causal);
+  if (Hkv <= 0 || H % Hkv != 0)
+    return fail(B200_EINVAL, "fmha_seqlens: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
+  if (num_splits < 0 || num_splits > kMaxSplits)
+    return fail(B200_EINVAL, "fmha_seqlens: num_splits=%d must be in 0 .. %d", num_splits, kMaxSplits);
+  if (static_cast<long long>(B) * Hkv > 65535)
+    return fail(B200_EINVAL, "fmha_seqlens: B*Hkv = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
+  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
+    return fail(B200_EINVAL,
+                "fmha_seqlens: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)");
+  if (static_cast<long long>(H / Hkv) * Nq > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "fmha_seqlens: (H/Hkv)*Nq = %lld query rows per K/V head exceed 2^31 - 1",
+                static_cast<long long>(H / Hkv) * Nq);
+  if ((reinterpret_cast<uintptr_t>(seqlens_q) & 3u) != 0)
+    return fail(B200_EINVAL, "fmha_seqlens: seqlens_q must be 4-byte aligned (int32)");
+  if ((reinterpret_cast<uintptr_t>(seqlens_k) & 3u) != 0)
+    return fail(B200_EINVAL, "fmha_seqlens: seqlens_k must be 4-byte aligned (int32)");
+  if (D % 8 != 0) return fail(B200_ENOTSUP, "fmha_seqlens: headdim not support! (D=%d must be a multiple of 8)", D);
+  if (D > 1024) return fail(B200_ENOTSUP, "fmha_seqlens: headdim not support! (D=%d > 1024)", D);
+  if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
+  const int G = H / Hkv;
+  // the split count follows the padded shape, as for b200_fmha_fwd_f16_gqa: the lengths stay on the device (and
+  // b200_fmha_fwd_f16_gqa_splits gives it for either element type)
+  const int splits = num_splits == 0 ? auto_splits(B, Hkv, G, Nq, Nk, D) : num_splits;
+  const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
+  return fmha_run<T>(q, k, v, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
+                  static_cast<cudaStream_t>(stream), &lens);
+}
+
+template <typename T>
+int fmha_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
+                            const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv,
+                            int Nq, int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
+                            int num_splits, float scale, void* stream) {
+  if (!q || !k_cache || !v_cache || !o || !block_table)
+    return fail(B200_EINVAL, "fmha_paged: null pointer (q, k_cache, v_cache, o and block_table are required)");
+  if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "fmha_paged: bad shape B=%d H=%d D=%d", B, H, D);
+  if (Nq <= 0) return fail(B200_EINVAL, "fmha_paged: bad length Nq=%d (must be >= 1)", Nq);
+  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_paged: causal must be 0 or 1, got %d", causal);
+  if (Hkv <= 0 || H % Hkv != 0)
+    return fail(B200_EINVAL, "fmha_paged: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
+  if (num_splits < 0 || num_splits > kMaxSplits)
+    return fail(B200_EINVAL, "fmha_paged: num_splits=%d must be in 0 .. %d", num_splits, kMaxSplits);
+  if (static_cast<long long>(B) * Hkv > 65535)
+    return fail(B200_EINVAL, "fmha_paged: B*Hkv = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
+  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
+    return fail(B200_EINVAL,
+                "fmha_paged: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)");
+  if (static_cast<long long>(H / Hkv) * Nq > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "fmha_paged: (H/Hkv)*Nq = %lld query rows per K/V head exceed 2^31 - 1",
+                static_cast<long long>(H / Hkv) * Nq);
+  if ((reinterpret_cast<uintptr_t>(seqlens_q) & 3u) != 0)
+    return fail(B200_EINVAL, "fmha_paged: seqlens_q must be 4-byte aligned (int32)");
+  if ((reinterpret_cast<uintptr_t>(seqlens_k) & 3u) != 0)
+    return fail(B200_EINVAL, "fmha_paged: seqlens_k must be 4-byte aligned (int32)");
+  if ((reinterpret_cast<uintptr_t>(block_table) & 3u) != 0)
+    return fail(B200_EINVAL, "fmha_paged: block_table must be 4-byte aligned (int32)");
+  if (num_pages < 1) return fail(B200_EINVAL, "fmha_paged: num_pages=%d must be >= 1", num_pages);
+  if (max_pages_per_seq < 1)
+    return fail(B200_EINVAL, "fmha_paged: max_pages_per_seq=%d must be >= 1", max_pages_per_seq);
+  if (page_size < 16 || (page_size & (page_size - 1)) != 0)
+    return fail(B200_EINVAL, "fmha_paged: page_size=%d must be a power of two >= 16", page_size);
+  if (static_cast<long long>(num_pages) * page_size > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "fmha_paged: num_pages*page_size = %lld pool rows exceed 2^31 - 1",
+                static_cast<long long>(num_pages) * page_size);
+  if (static_cast<long long>(max_pages_per_seq) * page_size > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "fmha_paged: max_pages_per_seq*page_size = %lld keys per sequence exceed 2^31 - 1",
+                static_cast<long long>(max_pages_per_seq) * page_size);
+  if (D % 8 != 0) return fail(B200_ENOTSUP, "fmha_paged: headdim not support! (D=%d must be a multiple of 8)", D);
+  if (D > 1024) return fail(B200_ENOTSUP, "fmha_paged: headdim not support! (D=%d > 1024)", D);
+  if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
+  const int G = H / Hkv, Nk = max_pages_per_seq * page_size;
+  // everything but the K/V addressing is the seqlens call on the padded Nk, the split count included
+  const int splits = num_splits == 0 ? auto_splits(B, Hkv, G, Nq, Nk, D) : num_splits;
+  const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
+  const attn::Pages pages{block_table, page_size, max_pages_per_seq};
+  return fmha_run<T>(q, k_cache, v_cache, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
+                  static_cast<cudaStream_t>(stream), &lens, &pages, num_pages);
 }
 
 }  // namespace
@@ -402,86 +481,31 @@ int b200_fmha_fwd_f16_gqa_splits(int B, int H, int Hkv, int Nq, int Nk, int D) {
 int b200_fmha_fwd_f16_seqlens(const void* q, const void* k, const void* v, void* o, float* lse, const int* seqlens_q,
                               const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk, int D, int causal,
                               int num_splits, float scale, void* stream) {
-  if (!q || !k || !v || !o) return fail(B200_EINVAL, "fmha_seqlens: null pointer (q, k, v and o are required)");
-  if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "fmha_seqlens: bad shape B=%d H=%d D=%d", B, H, D);
-  if (Nq <= 0 || Nk <= 0)
-    return fail(B200_EINVAL, "fmha_seqlens: bad lengths Nq=%d Nk=%d (both must be >= 1)", Nq, Nk);
-  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_seqlens: causal must be 0 or 1, got %d", causal);
-  if (Hkv <= 0 || H % Hkv != 0)
-    return fail(B200_EINVAL, "fmha_seqlens: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
-  if (num_splits < 0 || num_splits > kMaxSplits)
-    return fail(B200_EINVAL, "fmha_seqlens: num_splits=%d must be in 0 .. %d", num_splits, kMaxSplits);
-  if (static_cast<long long>(B) * Hkv > 65535)
-    return fail(B200_EINVAL, "fmha_seqlens: B*Hkv = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
-  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
-    return fail(B200_EINVAL,
-                "fmha_seqlens: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)");
-  if (static_cast<long long>(H / Hkv) * Nq > 0x7FFFFFFFll)
-    return fail(B200_EINVAL, "fmha_seqlens: (H/Hkv)*Nq = %lld query rows per K/V head exceed 2^31 - 1",
-                static_cast<long long>(H / Hkv) * Nq);
-  if ((reinterpret_cast<uintptr_t>(seqlens_q) & 3u) != 0)
-    return fail(B200_EINVAL, "fmha_seqlens: seqlens_q must be 4-byte aligned (int32)");
-  if ((reinterpret_cast<uintptr_t>(seqlens_k) & 3u) != 0)
-    return fail(B200_EINVAL, "fmha_seqlens: seqlens_k must be 4-byte aligned (int32)");
-  if (D % 8 != 0) return fail(B200_ENOTSUP, "fmha_seqlens: headdim not support! (D=%d must be a multiple of 8)", D);
-  if (D > 1024) return fail(B200_ENOTSUP, "fmha_seqlens: headdim not support! (D=%d > 1024)", D);
-  if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
-  const int G = H / Hkv;
-  // the split count follows the padded shape, as for b200_fmha_fwd_f16_gqa: the lengths stay on the device
-  const int splits = num_splits == 0 ? auto_splits(B, Hkv, G, Nq, Nk, D) : num_splits;
-  const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
-  return fmha_run(q, k, v, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
-                  static_cast<cudaStream_t>(stream), &lens);
+  return fmha_seqlens<__half>(q, k, v, o, lse, seqlens_q, seqlens_k, B, H, Hkv, Nq, Nk, D, causal, num_splits, scale,
+                              stream);
 }
 
 int b200_fmha_fwd_f16_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
                             const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv,
                             int Nq, int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
                             int num_splits, float scale, void* stream) {
-  if (!q || !k_cache || !v_cache || !o || !block_table)
-    return fail(B200_EINVAL, "fmha_paged: null pointer (q, k_cache, v_cache, o and block_table are required)");
-  if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "fmha_paged: bad shape B=%d H=%d D=%d", B, H, D);
-  if (Nq <= 0) return fail(B200_EINVAL, "fmha_paged: bad length Nq=%d (must be >= 1)", Nq);
-  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_paged: causal must be 0 or 1, got %d", causal);
-  if (Hkv <= 0 || H % Hkv != 0)
-    return fail(B200_EINVAL, "fmha_paged: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
-  if (num_splits < 0 || num_splits > kMaxSplits)
-    return fail(B200_EINVAL, "fmha_paged: num_splits=%d must be in 0 .. %d", num_splits, kMaxSplits);
-  if (static_cast<long long>(B) * Hkv > 65535)
-    return fail(B200_EINVAL, "fmha_paged: B*Hkv = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
-  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
-    return fail(B200_EINVAL,
-                "fmha_paged: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)");
-  if (static_cast<long long>(H / Hkv) * Nq > 0x7FFFFFFFll)
-    return fail(B200_EINVAL, "fmha_paged: (H/Hkv)*Nq = %lld query rows per K/V head exceed 2^31 - 1",
-                static_cast<long long>(H / Hkv) * Nq);
-  if ((reinterpret_cast<uintptr_t>(seqlens_q) & 3u) != 0)
-    return fail(B200_EINVAL, "fmha_paged: seqlens_q must be 4-byte aligned (int32)");
-  if ((reinterpret_cast<uintptr_t>(seqlens_k) & 3u) != 0)
-    return fail(B200_EINVAL, "fmha_paged: seqlens_k must be 4-byte aligned (int32)");
-  if ((reinterpret_cast<uintptr_t>(block_table) & 3u) != 0)
-    return fail(B200_EINVAL, "fmha_paged: block_table must be 4-byte aligned (int32)");
-  if (num_pages < 1) return fail(B200_EINVAL, "fmha_paged: num_pages=%d must be >= 1", num_pages);
-  if (max_pages_per_seq < 1)
-    return fail(B200_EINVAL, "fmha_paged: max_pages_per_seq=%d must be >= 1", max_pages_per_seq);
-  if (page_size < 16 || (page_size & (page_size - 1)) != 0)
-    return fail(B200_EINVAL, "fmha_paged: page_size=%d must be a power of two >= 16", page_size);
-  if (static_cast<long long>(num_pages) * page_size > 0x7FFFFFFFll)
-    return fail(B200_EINVAL, "fmha_paged: num_pages*page_size = %lld pool rows exceed 2^31 - 1",
-                static_cast<long long>(num_pages) * page_size);
-  if (static_cast<long long>(max_pages_per_seq) * page_size > 0x7FFFFFFFll)
-    return fail(B200_EINVAL, "fmha_paged: max_pages_per_seq*page_size = %lld keys per sequence exceed 2^31 - 1",
-                static_cast<long long>(max_pages_per_seq) * page_size);
-  if (D % 8 != 0) return fail(B200_ENOTSUP, "fmha_paged: headdim not support! (D=%d must be a multiple of 8)", D);
-  if (D > 1024) return fail(B200_ENOTSUP, "fmha_paged: headdim not support! (D=%d > 1024)", D);
-  if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
-  const int G = H / Hkv, Nk = max_pages_per_seq * page_size;
-  // everything but the K/V addressing is b200_fmha_fwd_f16_seqlens on the padded Nk, the split count included
-  const int splits = num_splits == 0 ? auto_splits(B, Hkv, G, Nq, Nk, D) : num_splits;
-  const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
-  const attn::Pages pages{block_table, page_size, max_pages_per_seq};
-  return fmha_run(q, k_cache, v_cache, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
-                  static_cast<cudaStream_t>(stream), &lens, &pages, num_pages);
+  return fmha_paged<__half>(q, k_cache, v_cache, o, lse, block_table, seqlens_q, seqlens_k, B, H, Hkv, Nq, num_pages,
+                            page_size, max_pages_per_seq, D, causal, num_splits, scale, stream);
+}
+
+int b200_fmha_fwd_bf16_seqlens(const void* q, const void* k, const void* v, void* o, float* lse, const int* seqlens_q,
+                               const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk, int D, int causal,
+                               int num_splits, float scale, void* stream) {
+  return fmha_seqlens<__nv_bfloat16>(q, k, v, o, lse, seqlens_q, seqlens_k, B, H, Hkv, Nq, Nk, D, causal, num_splits,
+                                     scale, stream);
+}
+
+int b200_fmha_fwd_bf16_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
+                             const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv,
+                             int Nq, int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
+                             int num_splits, float scale, void* stream) {
+  return fmha_paged<__nv_bfloat16>(q, k_cache, v_cache, o, lse, block_table, seqlens_q, seqlens_k, B, H, Hkv, Nq,
+                                   num_pages, page_size, max_pages_per_seq, D, causal, num_splits, scale, stream);
 }
 
 int b200_fmha_fwd_f16_rmsnorm(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H,

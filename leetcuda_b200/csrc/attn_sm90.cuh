@@ -61,6 +61,8 @@
 #pragma once
 #include <cuda.h>
 
+#include <type_traits>
+
 #include "softmax_math.cuh"
 
 namespace b200 {
@@ -77,7 +79,7 @@ struct Params {
   float* lse;          // [B*H, Nq] natural-log LSE, or nullptr
   float rms_g;         // > 0: RMS-normalise every output row; with several slabs the CTAs of a query tile form
                        // a cluster and add up the row statistics through distributed shared memory
-  __half* o_ptr;
+  __half* o_ptr;       // the output, of the kernel's element type (__half or __nv_bfloat16)
   float* ws_o;         // kSplit: [splits, B*H*Nq', D] fp32 normalised O of every split
   float* ws_lse;       //                          [splits, B*H*Nq'] natural-log LSE of every split
   int qpos;            // kGQA: query positions per head (the call's Nq); packed row r has position r % qpos
@@ -177,14 +179,23 @@ __device__ __forceinline__ int2 kv_blocks(const Params& p, int q0, int row_end, 
 // kDS: columns of O per CTA (64, 128 or 256); kBN: keys per block; kVT: V is [B,H,D,N]; kCausal: the causal mask;
 // kGQA: the causal mask on packed query heads; kSplit: split-KV; kSeqlens: per-sequence lengths from `lens` (see the top
 // of this file); kPaged: K and V in pages of a pool through `pages` (implies kSeqlens).  kCausal, kGQA, kSplit, kSeqlens
-// and kPaged are template parameters so that the other kernels compile to the code they had without them.
-template <int kDS, int kBN, int kWG, bool kVT, bool kCausal, bool kGQA, bool kSplit, bool kSeqlens, bool kPaged = false>
+// and kPaged are template parameters so that the other kernels compile to the code they had without them.  T: the
+// element type of Q, K, V and O, __half or __nv_bfloat16 (the top of this file; natural V only for bf16).
+template <int kDS, int kBN, int kWG, bool kVT, bool kCausal, bool kGQA, bool kSplit, bool kSeqlens, bool kPaged = false,
+          typename T = __half>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k,
                                               const CUtensorMap& tmap_v, Params p, const Lens& lens,
                                               const Pages& pages = Pages{}) {
   static_assert(!kVT || kDS <= 128, "transposed V: one slab of <= 128 columns");
   static_assert(!kSeqlens || (!kVT && kGQA), "per-sequence lengths: natural V, query positions of packed rows");
   static_assert(!kPaged || kSeqlens, "paged K/V: per-sequence lengths");
+  constexpr bool kBF16 = std::is_same_v<T, __nv_bfloat16>;
+  static_assert(kBF16 || std::is_same_v<T, __half>, "elements: fp16 or bf16");
+  static_assert(!kBF16 || !kVT, "bf16: natural V");
+  auto pack = [](float lo, float hi) {   // two fp32 values rounded to T (P, O)
+    if constexpr (kBF16) return pack_bf162(lo, hi);
+    else return pack_half2(lo, hi);
+  };
   constexpr int SLOT = slot_bytes(kBN, kDS, kVT);
   constexpr int KV_BYTES = 64 * kBN * 2;   // one {64 columns, kBN keys} chunk of K or V
   constexpr int NS = kBN / 2;     // S accumulator registers per thread
@@ -411,7 +422,9 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
       for (int ks = 0; ks < 4; ++ks) {
         const uint64_t da = wg_desc(qa + ks * 32, 16), db = wg_desc(ka + ks * 32, 16);
         const uint32_t go = (c > 0 || ks > 0) ? 1u : 0u;
-        if constexpr (kBN == 128) wgmma_ss_m64n128k16_f32_f16<0, 0>(s, da, db, go);
+        if constexpr (kBF16 && kBN == 128) wgmma_ss_m64n128k16_f32_bf16<0, 0>(s, da, db, go);
+        else if constexpr (kBF16) wgmma_ss_m64n64k16_f32_bf16<0, 0>(s, da, db, go);
+        else if constexpr (kBN == 128) wgmma_ss_m64n128k16_f32_f16<0, 0>(s, da, db, go);
         else wgmma_ss_m64n64k16_f32_f16<0, 0>(s, da, db, go);
       }
       wg_commit();
@@ -482,14 +495,14 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
         o[c][4 * jj + 2] *= alpha[1];
         o[c][4 * jj + 3] *= alpha[1];
       }
-    // P (fp16) as the A fragments of the k16 steps over the keys of this block
+    // P (rounded to T) as the A fragments of the k16 steps over the keys of this block
     uint32_t pa[kBN / 16][4];
 #pragma unroll
     for (int kk = 0; kk < kBN / 16; ++kk) {
-      pa[kk][0] = pack_half2(s[8 * kk + 0], s[8 * kk + 1]);
-      pa[kk][1] = pack_half2(s[8 * kk + 2], s[8 * kk + 3]);
-      pa[kk][2] = pack_half2(s[8 * kk + 4], s[8 * kk + 5]);
-      pa[kk][3] = pack_half2(s[8 * kk + 6], s[8 * kk + 7]);
+      pa[kk][0] = pack(s[8 * kk + 0], s[8 * kk + 1]);
+      pa[kk][1] = pack(s[8 * kk + 2], s[8 * kk + 3]);
+      pa[kk][2] = pack(s[8 * kk + 4], s[8 * kk + 5]);
+      pa[kk][3] = pack(s[8 * kk + 6], s[8 * kk + 7]);
     }
 
     // ---- O += P V over the slab's V chunks
@@ -509,8 +522,10 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
       } else {
         // chunk c = columns d0 + 64c .. +63 for all kBN keys (MN-major)
 #pragma unroll
-        for (int kk = 0; kk < kBN / 16; ++kk)
-          wgmma_rs_m64n64k16_f32_f16<1>(o[c], pa[kk], wg_desc(va + kk * 2048, 8192), 1u);
+        for (int kk = 0; kk < kBN / 16; ++kk) {
+          if constexpr (kBF16) wgmma_rs_m64n64k16_f32_bf16<1>(o[c], pa[kk], wg_desc(va + kk * 2048, 8192), 1u);
+          else wgmma_rs_m64n64k16_f32_f16<1>(o[c], pa[kk], wg_desc(va + kk * 2048, 8192), 1u);
+        }
       }
       wg_commit();
       wg_wait<1>();
@@ -609,7 +624,7 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj) {
             const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
-            if (col < p.D) *reinterpret_cast<uint32_t*>(p.o_ptr + (head + row) * p.D + col) = 0u;
+            if (col < p.D) *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.o_ptr) + (head + row) * p.D + col) = 0u;
           }
         continue;
       }
@@ -617,15 +632,14 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
     if (p.lse && slab == 0 && (lane % 4) == 0)
       p.lse[head + row] =
           kCausal && m[i] == -INFINITY ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
-    __half* orow = p.o_ptr + (head + row) * p.D;
+    T* orow = reinterpret_cast<T*>(p.o_ptr) + (head + row) * p.D;
 #pragma unroll
     for (int c = 0; c < NDC; ++c)
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) {
         const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
         if (col < p.D)
-          *reinterpret_cast<uint32_t*>(orow + col) =
-              pack_half2(o[c][4 * jj + 2 * i] * inv[i], o[c][4 * jj + 2 * i + 1] * inv[i]);
+          *reinterpret_cast<uint32_t*>(orow + col) = pack(o[c][4 * jj + 2 * i] * inv[i], o[c][4 * jj + 2 * i + 1] * inv[i]);
       }
   }
 }
@@ -651,6 +665,25 @@ __global__ void __launch_bounds__(threads<kWG>(), 1)
 attn_fwd_paged_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                       const __grid_constant__ CUtensorMap tmap_v, const Params p, const Lens lens, const Pages pages) {
   attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, kSplit, true, true>(tmap_q, tmap_k, tmap_v, p, lens, pages);
+}
+
+// bf16 Q, K, V and O (b200_fmha_fwd_bf16_seqlens, b200_fmha_fwd_bf16_paged): the two kernels above with bf16 elements.
+// A dense bf16 call runs attn_fwd_seqlens_bf16_kernel with null length arrays.  Instantiated in attn_bf16.cu.
+template <int kDS, int kBN, int kWG, bool kCausal, bool kSplit>
+__global__ void __launch_bounds__(threads<kWG>(), 1)
+attn_fwd_seqlens_bf16_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                             const __grid_constant__ CUtensorMap tmap_v, const Params p, const Lens lens) {
+  attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, kSplit, true, false, __nv_bfloat16>(tmap_q, tmap_k, tmap_v, p,
+                                                                                         lens);
+}
+
+template <int kDS, int kBN, int kWG, bool kCausal, bool kSplit>
+__global__ void __launch_bounds__(threads<kWG>(), 1)
+attn_fwd_paged_bf16_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                           const __grid_constant__ CUtensorMap tmap_v, const Params p, const Lens lens,
+                           const Pages pages) {
+  attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, kSplit, true, true, __nv_bfloat16>(tmap_q, tmap_k, tmap_v, p, lens,
+                                                                                        pages);
 }
 
 }  // namespace attn

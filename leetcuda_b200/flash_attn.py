@@ -65,12 +65,10 @@ V_TRANSPOSED_OPS = {
 OP_NAMES = _BASIC + _ACC_F32 + _SWIZZLE + _OTHERS
 
 
-def _shapes(Q, K, V, O, v_transposed, same_length, grouped=False):
+def _shapes(Q, K, V, O, v_transposed, same_length, grouped=False, dtype=torch.float16):
     """(B, H, Nq, Nk, D, Hkv) of q, o [B,H,Nq,D], k [B,Hkv,Nk,D], v [B,Hkv,Nk,D] or [B,Hkv,D,Nk]; Nk = Nq if
     same_length; Hkv = H unless grouped, where any Hkv dividing H is accepted."""
-    for t in (Q, K, V, O):
-        if t.dtype != torch.float16:
-            raise RuntimeError("values must be torch::kHalf")
+    _check_dtype(Q, K, V, O, dtype)
     if Q.dim() != 4 or K.dim() != 4:
         raise RuntimeError("Tensor size mismatch!")
     B, H, Nq, D = Q.shape
@@ -82,6 +80,23 @@ def _shapes(Q, K, V, O, v_transposed, same_length, grouped=False):
     if tuple(V.shape) != want_v:
         raise RuntimeError("Tensor size mismatch!")
     return B, H, Nq, Nk, D, Hkv
+
+
+def _check_dtype(Q, K, V, O, dtype):
+    for t in (Q, K, V, O):
+        if t.dtype != dtype:
+            raise RuntimeError("values must be torch::kHalf" if dtype == torch.float16 else "values must be torch::kBFloat16")
+
+
+def _element_type(Q, K, V, O):
+    """torch.bfloat16 when Q, K, V and O are all bf16, else torch.float16 (whose checks reject any other dtype)."""
+    dts = [t.dtype for t in (Q, K, V, O)]
+    if torch.bfloat16 not in dts:
+        return torch.float16
+    if any(d != torch.bfloat16 for d in dts):
+        raise RuntimeError("leetcuda_b200.flash_attn: Q, K, V and O must share one dtype (all fp16 or all bf16), got "
+                           + ", ".join(str(d).replace("torch.", "") for d in dts))
+    return torch.bfloat16
 
 
 def _placement(*tensors):
@@ -132,12 +147,20 @@ def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=
     ``Nk = max_pages_per_seq * page_size`` keys, bit for bit, without gathering the pages.  Table entries past a
     sequence's last used page are never read (pad with -1 or stale ids); pages may be shared between sequences.  The
     table is read on the GPU only, so a captured graph replays with whatever tables and lengths the tensors hold.
-    page_size must be a power of two >= 16; natural V only."""
+    page_size must be a power of two >= 16; natural V only.
+
+    Q, K, V and O are all fp16 or all bf16 (``torch.bfloat16``: ``b200_fmha_fwd_bf16_seqlens`` / ``_paged``, every option
+    above but ``v_transposed``; lse stays fp32).  A bf16 call rounds P and O to bf16 where an fp16 one rounds them to fp16
+    and is otherwise the same computation; a bf16 call without lengths runs the per-sequence-length kernel with every
+    sequence at Nq / Nk."""
+    dtype = _element_type(Q, K, V, O)
+    if dtype == torch.bfloat16 and v_transposed:
+        raise RuntimeError("leetcuda_b200.flash_attn: transposed V is fp16 only (v_transposed=True with bf16 tensors)")
     if block_table is not None:
-        _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table)
+        _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table, dtype)
         return
-    if seqlens_q is not None or seqlens_k is not None:
-        _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k)
+    if seqlens_q is not None or seqlens_k is not None or dtype == torch.bfloat16:
+        _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, dtype)
         return
     B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, v_transposed, same_length=False, grouped=True)
     if isinstance(num_splits, bool) or not isinstance(num_splits, int) or not 0 <= num_splits <= _capi.FMHA_MAX_SPLITS:
@@ -149,17 +172,19 @@ def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=
     _run(Q, K, V, O, B, H, Nq, Nk, D, v_transposed, scale, lse, causal, Hkv, num_splits)
 
 
-def _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k) -> None:
+def _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k,
+                  dtype=torch.float16) -> None:
     if v_transposed:
         raise RuntimeError("leetcuda_b200.flash_attn: seqlens_q / seqlens_k take natural V [B,Hkv,Nk,D] only "
                            "(v_transposed=True is not supported with lengths)")
-    B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, False, same_length=False, grouped=True)
+    B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, False, same_length=False, grouped=True, dtype=dtype)
     _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k)
     _placement(Q, K, V, O, *(() if lse is None else (lse,)))
     args = [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), None if lse is None else lse.data_ptr(),
             None if seqlens_q is None else seqlens_q.data_ptr(), None if seqlens_k is None else seqlens_k.data_ptr(),
             B, H, Hkv, Nq, Nk, D, int(bool(causal)), int(num_splits), float(scale)]
-    _call_on_device(_capi.lib().b200_fmha_fwd_f16_seqlens, args, Q.device.index)
+    fn = _capi.lib().b200_fmha_fwd_bf16_seqlens if dtype == torch.bfloat16 else _capi.lib().b200_fmha_fwd_f16_seqlens
+    _call_on_device(fn, args, Q.device.index)
 
 
 def _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k) -> None:
@@ -178,13 +203,12 @@ def _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k) -> None:
                                f"on Q's device")
 
 
-def _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table) -> None:
+def _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table,
+                dtype=torch.float16) -> None:
     if v_transposed:
         raise RuntimeError("leetcuda_b200.flash_attn: block_table takes natural V pools [num_pages,page_size,Hkv,D] "
                            "only (v_transposed=True is not supported with a block table)")
-    for t in (Q, K, V, O):
-        if t.dtype != torch.float16:
-            raise RuntimeError("values must be torch::kHalf")
+    _check_dtype(Q, K, V, O, dtype)
     if Q.dim() != 4 or tuple(O.shape) != tuple(Q.shape):
         raise RuntimeError("Tensor size mismatch!")
     B, H, Nq, D = Q.shape
@@ -207,7 +231,8 @@ def _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlen
             t.data_ptr(), None if seqlens_q is None else seqlens_q.data_ptr(),
             None if seqlens_k is None else seqlens_k.data_ptr(), B, H, Hkv, Nq, num_pages, page_size, t.shape[1], D,
             int(bool(causal)), int(num_splits), float(scale)]
-    _call_on_device(_capi.lib().b200_fmha_fwd_f16_paged, args, Q.device.index)
+    fn = _capi.lib().b200_fmha_fwd_bf16_paged if dtype == torch.bfloat16 else _capi.lib().b200_fmha_fwd_f16_paged
+    _call_on_device(fn, args, Q.device.index)
 
 
 def _call_on_device(fn, args, idx) -> None:

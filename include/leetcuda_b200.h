@@ -226,6 +226,36 @@ int b200_fmha_fwd_bf16_seqlens(const void* q, const void* k, const void* v, void
                                const int* seqlens_q /* may be NULL */, const int* seqlens_k /* may be NULL */,
                                int B, int H, int Hkv, int Nq, int Nk, int D, int causal, int num_splits, float scale,
                                void* stream);
+/* fp8 (OCP e4m3, torch.float8_e4m3fn) K and V with fp16 or bf16 q and o: the argument lists of
+ * b200_fmha_fwd_{f16,bf16}_seqlens and _paged plus k_scale and v_scale before stream; k, v (k_cache, v_cache) hold
+ * e4m3 bytes, [B, Hkv, Nk, D] resp. pools [num_pages, page_size, Hkv, D].  O = softmax(scale * Q (k_scale K)^T)
+ * (v_scale V) with every semantic of the counterpart (lengths, causal mask, GQA, split-KV, paging, padded rows).
+ * K and V are widened exactly to the type of q; k_scale is folded into the softmax scale as fp32(scale * k_scale)
+ * (scale <= 0 is first replaced by 1/sqrt(D)), and v_scale multiplies the normalised fp32 O (or each split's part)
+ * before O's one rounding; lse does not see v_scale.  With v_scale = 1 the call is bit for bit the counterpart on
+ * K and V converted to q's type with scale = fp32(scale * k_scale).
+ * Checks: exactly those of the counterpart with its codes and messages, then B200_EINVAL for D % 16 != 0 (an e4m3 row
+ * of D bytes is the TMA row stride), for k_scale or v_scale not finite and > 0, and for fp32(scale * k_scale) not
+ * finite and > 0. */
+int b200_fmha_fwd_f16_fp8kv_seqlens(const void* q, const void* k, const void* v, void* o, float* lse /* may be NULL */,
+                                    const int* seqlens_q /* may be NULL */, const int* seqlens_k /* may be NULL */,
+                                    int B, int H, int Hkv, int Nq, int Nk, int D, int causal, int num_splits,
+                                    float scale, float k_scale, float v_scale, void* stream);
+int b200_fmha_fwd_bf16_fp8kv_seqlens(const void* q, const void* k, const void* v, void* o, float* lse /* may be NULL */,
+                                     const int* seqlens_q /* may be NULL */, const int* seqlens_k /* may be NULL */,
+                                     int B, int H, int Hkv, int Nq, int Nk, int D, int causal, int num_splits,
+                                     float scale, float k_scale, float v_scale, void* stream);
+int b200_fmha_fwd_f16_fp8kv_paged(const void* q, const void* k_cache, const void* v_cache, void* o,
+                                  float* lse /* may be NULL */, const int* block_table,
+                                  const int* seqlens_q /* may be NULL */, const int* seqlens_k /* may be NULL */, int B,
+                                  int H, int Hkv, int Nq, int num_pages, int page_size, int max_pages_per_seq, int D,
+                                  int causal, int num_splits, float scale, float k_scale, float v_scale, void* stream);
+int b200_fmha_fwd_bf16_fp8kv_paged(const void* q, const void* k_cache, const void* v_cache, void* o,
+                                   float* lse /* may be NULL */, const int* block_table,
+                                   const int* seqlens_q /* may be NULL */, const int* seqlens_k /* may be NULL */,
+                                   int B, int H, int Hkv, int Nq, int num_pages, int page_size, int max_pages_per_seq,
+                                   int D, int causal, int num_splits, float scale, float k_scale, float v_scale,
+                                   void* stream);
 int b200_fmha_fwd_bf16_paged(const void* q, const void* k_cache, const void* v_cache, void* o,
                              float* lse /* may be NULL */, const int* block_table,
                              const int* seqlens_q /* may be NULL */, const int* seqlens_k /* may be NULL */, int B,

@@ -8,6 +8,8 @@
 
 #include <type_traits>
 
+#include <cuda_fp8.h>
+
 #include "attn_launch.cuh"
 
 namespace {
@@ -159,12 +161,15 @@ Family family(int D) {
 // G: query heads per K/V head (H = G * Hkv; the kernel sees B * Hkv heads of G * Nq packed rows).  splits > 1: grid.z
 // splits whose fp32 parts go to ws_o / ws_lse instead of o / lse (kSplit kernels).  Causal with G > 1 runs kGQA.
 // pages: k and v are pools of num_pages pages [page_size, Hkv, D], and Nk is the padded max_pages * page_size.
-// T: the element type of q, k, v and o; __nv_bfloat16 runs the bf16 kernels (attn_bf16.cu), which take lens always.
-template <typename T>
+// T: the element type of q and o, KV that of k and v: T (__nv_bfloat16 runs the bf16 kernels, attn_bf16.cu) or
+// __nv_fp8_e4m3 (the fp8-K/V kernels, attn_fp8kv_*.cu, with v_scale); both take lens always.
+template <typename T, typename KV = T>
 int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int Hkv, int G,
                   int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, float* ws_o, float* ws_lse,
                   cudaStream_t stream, const attn::Lens* lens = nullptr, const attn::Pages* pages = nullptr,
-                  int num_pages = 0) {
+                  int num_pages = 0, float v_scale = 1.f) {
+  constexpr bool fp8 = std::is_same_v<KV, __nv_fp8_e4m3>;
+  static_assert(fp8 || std::is_same_v<KV, T>, "K/V: the element type of Q and O, or e4m3");
   const uint64_t BH = static_cast<uint64_t>(B) * Hkv;
   const Family f = family(D);
   const int ds = f.ds, bn = f.bn, wgs = f.wgs;
@@ -190,21 +195,27 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
   const int kMaxSmem = 227 * 1024;
   const int slot = attn::slot_bytes(bn, ds, vt);
   const int fixed = attn::smem_bytes(wgs, slot, p.nq, 0);
-  p.ring = (kMaxSmem - fixed) / (slot + 16);
+  // fp8: every ring slot has a staging chunk of e4m3 bytes and its barrier beside it (attn_sm90.cuh)
+  const int stage = fp8 ? 64 * bn + 8 : 0;
+  p.ring = (kMaxSmem - fixed) / (slot + 16 + stage);
   if (p.ring > 16) p.ring = 16;
   if (p.ring < 2) return fail(B200_ENOTSUP, "headdim not support! (D=%d)", D);
-  const int smem = attn::smem_bytes(wgs, slot, p.nq, p.ring);
+  const int smem = attn::smem_bytes(wgs, slot, p.nq, p.ring) + p.ring * stage;
   // causal packed heads of at least one tile of rows: tiles of their own per head (attn_sm90.cuh), else packed tiles
   p.tph = causal && Nq >= 64 * wgs ? (Nq + 64 * wgs - 1) / (64 * wgs) : 0;
   const int qtiles = p.tph > 0 ? G * p.tph : (rows + 64 * wgs - 1) / (64 * wgs);
 
   constexpr bool bf16 = std::is_same_v<T, __nv_bfloat16>;
   const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  // fp8: K and V rows of D bytes, staged unswizzled (the converters write the 128B-swizzled T rows)
+  const CUtensorMapDataType kvdt = fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : dt;
+  const CUtensorMapSwizzle kvsw = fp8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
+  const uint64_t kveb = sizeof(KV);
   CUtensorMap tq, tk, tv;
   uint64_t qdims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(rows), BH};
   uint64_t qstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(rows) * D * 2};
   uint64_t kdims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(Nk), BH};
-  uint64_t kstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(Nk) * D * 2};
+  uint64_t kstr[2] = {static_cast<uint64_t>(D) * kveb, static_cast<uint64_t>(Nk) * D * kveb};
   uint32_t qbox[3] = {64, 64, 1};
   uint32_t kbox[3] = {64, static_cast<uint32_t>(bn), 1};
   int rc;
@@ -213,26 +224,36 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
     // pool rows {D, Hkv, num_pages * page_size}; a key block is kBN / R boxes of R = min(page_size, kBN) rows
     uint64_t pd[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(Hkv),
                       static_cast<uint64_t>(num_pages) * static_cast<uint64_t>(pages->page_size)};
-    uint64_t pstr[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(Hkv) * D * 2};
+    uint64_t pstr[2] = {static_cast<uint64_t>(D) * kveb, static_cast<uint64_t>(Hkv) * D * kveb};
     uint32_t pbox[3] = {64, 1, static_cast<uint32_t>(std::min(pages->page_size, bn))};
-    if ((rc = host::get_tmap(&tk, k, 3, pd, pstr, pbox, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
-    if ((rc = host::get_tmap(&tv, v, 3, pd, pstr, pbox, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
+    if ((rc = host::get_tmap(&tk, k, 3, pd, pstr, pbox, kvsw, kvdt))) return rc;
+    if ((rc = host::get_tmap(&tv, v, 3, pd, pstr, pbox, kvsw, kvdt))) return rc;
   } else {
-    if ((rc = host::get_tmap(&tk, k, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
+    if ((rc = host::get_tmap(&tk, k, 3, kdims, kstr, kbox, kvsw, kvdt))) return rc;
     if (vt) {
       uint64_t vd[3] = {static_cast<uint64_t>(Nk), static_cast<uint64_t>(D), BH};
       uint64_t vs[2] = {static_cast<uint64_t>(Nk) * 2, static_cast<uint64_t>(Nk) * D * 2};
       uint32_t vb[3] = {64, static_cast<uint32_t>(ds), 1};
       if ((rc = host::get_tmap(&tv, v, 3, vd, vs, vb, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
     } else {
-      if ((rc = host::get_tmap(&tv, v, 3, kdims, kstr, kbox, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
+      if ((rc = host::get_tmap(&tv, v, 3, kdims, kstr, kbox, kvsw, kvdt))) return rc;
     }
   }
   const int bh = static_cast<int>(BH);
   if (vt && lens) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with lengths)");
   const bool pk = G > 1;
   const attn::Pages* pg = pages;
-  if constexpr (bf16) {
+  if constexpr (fp8) {
+    if (vt || !lens) return fail(B200_EINVAL, "fmha: internal dispatch error (fp8 K/V without lengths or with V^T)");
+    if (ds == 64)
+      return attn::launch_attn_fp8kv<T, 64, 128, 2>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, v_scale,
+                                                    stream);
+    if (ds == 128)
+      return attn::launch_attn_fp8kv<T, 128, 64, 2>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, v_scale,
+                                                    stream);
+    return attn::launch_attn_fp8kv<T, 256, 64, 1>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, v_scale,
+                                                  stream);
+  } else if constexpr (bf16) {
     if (vt || !lens) return fail(B200_EINVAL, "fmha: internal dispatch error (bf16 without lengths or with V^T)");
     if (ds == 64) return attn::launch_attn_bf16<64, 128, 2>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, stream);
     if (ds == 128) return attn::launch_attn_bf16<128, 64, 2>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, stream);
@@ -247,21 +268,22 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
 }
 
 // The attention kernel, and with splits > 1 its fp32 parts in a stream-ordered workspace and the combine kernel.
-template <typename T>
+template <typename T, typename KV = T>
 int fmha_run(const void* q, const void* k, const void* v, void* o, float* lse, float rms_g, int B, int Hkv, int G,
              int Nq, int Nk, int D, bool vt, bool causal, float scale, int splits, cudaStream_t stream,
-             const attn::Lens* lens = nullptr, const attn::Pages* pages = nullptr, int num_pages = 0) {
+             const attn::Lens* lens = nullptr, const attn::Pages* pages = nullptr, int num_pages = 0,
+             float v_scale = 1.f) {
   if (splits <= 1)
-    return fmha_dispatch<T>(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, 1, nullptr, nullptr, stream,
-                         lens, pages, num_pages);
+    return fmha_dispatch<T, KV>(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, 1, nullptr, nullptr,
+                                stream, lens, pages, num_pages, v_scale);
   const size_t rows = static_cast<size_t>(B) * Hkv * G * Nq;
   const size_t lse_bytes = (static_cast<size_t>(splits) * rows * 4 + 255) & ~static_cast<size_t>(255);
   void* ws = nullptr;
   B200_CUDA_OK(cudaMallocAsync(&ws, lse_bytes + static_cast<size_t>(splits) * rows * D * 4, stream));
   float* ws_lse = static_cast<float*>(ws);
   float* ws_o = reinterpret_cast<float*>(static_cast<char*>(ws) + lse_bytes);
-  int rc = fmha_dispatch<T>(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, splits, ws_o, ws_lse, stream,
-                         lens, pages, num_pages);
+  int rc = fmha_dispatch<T, KV>(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, vt, causal, scale, splits, ws_o, ws_lse,
+                                stream, lens, pages, num_pages, v_scale);
   if (rc == 0) rc = launch_combine(static_cast<T*>(o), lse, ws_o, ws_lse, rows, D, splits, stream);
   cudaFreeAsync(ws, stream);
   return rc;
@@ -335,11 +357,32 @@ int fmha_impl(const void* q, const void* k, const void* v, void* o, float* lse, 
   return fmha_run<__half>(q, k, v, o, lse, rms_g, B, Hkv, G, Nq, Nk, D, v_transposed != 0, causal, scale, splits, stream);
 }
 
-// b200_fmha_fwd_{f16,bf16}_seqlens and _paged: the same checks and messages for both element types T.
-template <typename T>
+// The fp8-K/V entries' own checks, after those of their counterparts (who: "fmha_seqlens" or "fmha_paged"), and the
+// softmax scale (defaulted as by the counterparts) with k_scale folded in: fp32(scale * k_scale), so that K elements
+// are never multiplied.
+int fp8kv_scales(const char* who, int D, float k_scale, float v_scale, float* scale) {
+  if (D % 16 != 0)
+    return fail(B200_EINVAL, "%s: fp8 K/V need D %% 16 == 0 (an e4m3 row of D bytes is the TMA row stride), got D=%d",
+                who, D);
+  if (!(isfinite(k_scale) && k_scale > 0.f))
+    return fail(B200_EINVAL, "%s: k_scale=%g must be finite and > 0", who, static_cast<double>(k_scale));
+  if (!(isfinite(v_scale) && v_scale > 0.f))
+    return fail(B200_EINVAL, "%s: v_scale=%g must be finite and > 0", who, static_cast<double>(v_scale));
+  if (!(*scale > 0.f)) *scale = 1.0f / sqrtf(static_cast<float>(D));
+  const float folded = *scale * k_scale;
+  if (!(isfinite(folded) && folded > 0.f))
+    return fail(B200_EINVAL, "%s: scale*k_scale = %g must be finite and > 0 in fp32", who,
+                static_cast<double>(folded));
+  *scale = folded;
+  return 0;
+}
+
+// b200_fmha_fwd_{f16,bf16}_seqlens and _paged: the same checks and messages for both element types T, and for the
+// fp8-K/V entries (KV = __nv_fp8_e4m3) with their own checks after these.
+template <typename T, typename KV = T>
 int fmha_seqlens(const void* q, const void* k, const void* v, void* o, float* lse, const int* seqlens_q,
                               const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk, int D, int causal,
-                              int num_splits, float scale, void* stream) {
+                              int num_splits, float scale, void* stream, float k_scale = 1.f, float v_scale = 1.f) {
   if (!q || !k || !v || !o) return fail(B200_EINVAL, "fmha_seqlens: null pointer (q, k, v and o are required)");
   if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "fmha_seqlens: bad shape B=%d H=%d D=%d", B, H, D);
   if (Nq <= 0 || Nk <= 0)
@@ -363,21 +406,24 @@ int fmha_seqlens(const void* q, const void* k, const void* v, void* o, float* ls
     return fail(B200_EINVAL, "fmha_seqlens: seqlens_k must be 4-byte aligned (int32)");
   if (D % 8 != 0) return fail(B200_ENOTSUP, "fmha_seqlens: headdim not support! (D=%d must be a multiple of 8)", D);
   if (D > 1024) return fail(B200_ENOTSUP, "fmha_seqlens: headdim not support! (D=%d > 1024)", D);
+  if constexpr (!std::is_same_v<KV, T>) {
+    if (int rc = fp8kv_scales("fmha_seqlens", D, k_scale, v_scale, &scale)) return rc;
+  }
   if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
   const int G = H / Hkv;
   // the split count follows the padded shape, as for b200_fmha_fwd_f16_gqa: the lengths stay on the device (and
   // b200_fmha_fwd_f16_gqa_splits gives it for either element type)
   const int splits = num_splits == 0 ? auto_splits(B, Hkv, G, Nq, Nk, D) : num_splits;
   const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
-  return fmha_run<T>(q, k, v, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
-                  static_cast<cudaStream_t>(stream), &lens);
+  return fmha_run<T, KV>(q, k, v, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
+                         static_cast<cudaStream_t>(stream), &lens, nullptr, 0, v_scale);
 }
 
-template <typename T>
+template <typename T, typename KV = T>
 int fmha_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
                             const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv,
                             int Nq, int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
-                            int num_splits, float scale, void* stream) {
+                            int num_splits, float scale, void* stream, float k_scale = 1.f, float v_scale = 1.f) {
   if (!q || !k_cache || !v_cache || !o || !block_table)
     return fail(B200_EINVAL, "fmha_paged: null pointer (q, k_cache, v_cache, o and block_table are required)");
   if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "fmha_paged: bad shape B=%d H=%d D=%d", B, H, D);
@@ -414,14 +460,17 @@ int fmha_paged(const void* q, const void* k_cache, const void* v_cache, void* o,
                 static_cast<long long>(max_pages_per_seq) * page_size);
   if (D % 8 != 0) return fail(B200_ENOTSUP, "fmha_paged: headdim not support! (D=%d must be a multiple of 8)", D);
   if (D > 1024) return fail(B200_ENOTSUP, "fmha_paged: headdim not support! (D=%d > 1024)", D);
+  if constexpr (!std::is_same_v<KV, T>) {
+    if (int rc = fp8kv_scales("fmha_paged", D, k_scale, v_scale, &scale)) return rc;
+  }
   if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
   const int G = H / Hkv, Nk = max_pages_per_seq * page_size;
   // everything but the K/V addressing is the seqlens call on the padded Nk, the split count included
   const int splits = num_splits == 0 ? auto_splits(B, Hkv, G, Nq, Nk, D) : num_splits;
   const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
   const attn::Pages pages{block_table, page_size, max_pages_per_seq};
-  return fmha_run<T>(q, k_cache, v_cache, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
-                  static_cast<cudaStream_t>(stream), &lens, &pages, num_pages);
+  return fmha_run<T, KV>(q, k_cache, v_cache, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
+                         static_cast<cudaStream_t>(stream), &lens, &pages, num_pages, v_scale);
 }
 
 }  // namespace
@@ -506,6 +555,41 @@ int b200_fmha_fwd_bf16_paged(const void* q, const void* k_cache, const void* v_c
                              int num_splits, float scale, void* stream) {
   return fmha_paged<__nv_bfloat16>(q, k_cache, v_cache, o, lse, block_table, seqlens_q, seqlens_k, B, H, Hkv, Nq,
                                    num_pages, page_size, max_pages_per_seq, D, causal, num_splits, scale, stream);
+}
+
+int b200_fmha_fwd_f16_fp8kv_seqlens(const void* q, const void* k, const void* v, void* o, float* lse,
+                                    const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk,
+                                    int D, int causal, int num_splits, float scale, float k_scale, float v_scale,
+                                    void* stream) {
+  return fmha_seqlens<__half, __nv_fp8_e4m3>(q, k, v, o, lse, seqlens_q, seqlens_k, B, H, Hkv, Nq, Nk, D, causal,
+                                             num_splits, scale, stream, k_scale, v_scale);
+}
+
+int b200_fmha_fwd_bf16_fp8kv_seqlens(const void* q, const void* k, const void* v, void* o, float* lse,
+                                     const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk,
+                                     int D, int causal, int num_splits, float scale, float k_scale, float v_scale,
+                                     void* stream) {
+  return fmha_seqlens<__nv_bfloat16, __nv_fp8_e4m3>(q, k, v, o, lse, seqlens_q, seqlens_k, B, H, Hkv, Nq, Nk, D, causal,
+                                                    num_splits, scale, stream, k_scale, v_scale);
+}
+
+int b200_fmha_fwd_f16_fp8kv_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
+                                  const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H,
+                                  int Hkv, int Nq, int num_pages, int page_size, int max_pages_per_seq, int D,
+                                  int causal, int num_splits, float scale, float k_scale, float v_scale, void* stream) {
+  return fmha_paged<__half, __nv_fp8_e4m3>(q, k_cache, v_cache, o, lse, block_table, seqlens_q, seqlens_k, B, H, Hkv,
+                                           Nq, num_pages, page_size, max_pages_per_seq, D, causal, num_splits, scale,
+                                           stream, k_scale, v_scale);
+}
+
+int b200_fmha_fwd_bf16_fp8kv_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
+                                   const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H,
+                                   int Hkv, int Nq, int num_pages, int page_size, int max_pages_per_seq, int D,
+                                   int causal, int num_splits, float scale, float k_scale, float v_scale,
+                                   void* stream) {
+  return fmha_paged<__nv_bfloat16, __nv_fp8_e4m3>(q, k_cache, v_cache, o, lse, block_table, seqlens_q, seqlens_k, B, H,
+                                                  Hkv, Nq, num_pages, page_size, max_pages_per_seq, D, causal,
+                                                  num_splits, scale, stream, k_scale, v_scale);
 }
 
 int b200_fmha_fwd_f16_rmsnorm(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H,

@@ -45,5 +45,12 @@ int launch_attn_bf16(const CUtensorMap& tq, const CUtensorMap& tk, const CUtenso
                      int BH, int smem, bool causal, int splits, const Lens& lens, const Pages* pages,
                      cudaStream_t stream);
 
+// The fp8-K/V kernel of the family (kDS, kBN, kWG) with T = __half or __nv_bfloat16 Q and O (attn_fp8kv_f16.cu,
+// attn_fp8kv_bf16.cu): attn_fwd_fp8kv_paged_kernel with pages, else attn_fwd_fp8kv_seqlens_kernel.
+template <typename T, int kDS, int kBN, int kWG>
+int launch_attn_fp8kv(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const Params& p, int qtiles,
+                      int BH, int smem, bool causal, int splits, const Lens& lens, const Pages* pages, float v_scale,
+                      cudaStream_t stream);
+
 }  // namespace attn
 }  // namespace b200

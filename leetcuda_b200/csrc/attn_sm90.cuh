@@ -181,14 +181,17 @@ __device__ __forceinline__ int2 kv_blocks(const Params& p, int q0, int row_end, 
 // of this file); kPaged: K and V in pages of a pool through `pages` (implies kSeqlens).  kCausal, kGQA, kSplit, kSeqlens
 // and kPaged are template parameters so that the other kernels compile to the code they had without them.  T: the
 // element type of Q, K, V and O, __half or __nv_bfloat16 (the top of this file; natural V only for bf16).
+// kFP8: K and V are e4m3 bytes, staged by TMA and widened to T in shared memory by producer warps 1-3 (the end of
+// this file); v_scale multiplies the normalised fp32 O before its rounding to T.
 template <int kDS, int kBN, int kWG, bool kVT, bool kCausal, bool kGQA, bool kSplit, bool kSeqlens, bool kPaged = false,
-          typename T = __half>
+          typename T = __half, bool kFP8 = false>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k,
                                               const CUtensorMap& tmap_v, Params p, const Lens& lens,
-                                              const Pages& pages = Pages{}) {
+                                              const Pages& pages = Pages{}, float v_scale = 1.f) {
   static_assert(!kVT || kDS <= 128, "transposed V: one slab of <= 128 columns");
   static_assert(!kSeqlens || (!kVT && kGQA), "per-sequence lengths: natural V, query positions of packed rows");
   static_assert(!kPaged || kSeqlens, "paged K/V: per-sequence lengths");
+  static_assert(!kFP8 || kSeqlens, "fp8 K/V: the per-sequence-length and paged kernels");
   constexpr bool kBF16 = std::is_same_v<T, __nv_bfloat16>;
   static_assert(kBF16 || std::is_same_v<T, __half>, "elements: fp16 or bf16");
   static_assert(!kBF16 || !kVT, "bf16: natural V");
@@ -198,6 +201,7 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
   };
   constexpr int SLOT = slot_bytes(kBN, kDS, kVT);
   constexpr int KV_BYTES = 64 * kBN * 2;   // one {64 columns, kBN keys} chunk of K or V
+  constexpr int STG = kFP8 ? 64 * kBN : 0;   // kFP8: one staged e4m3 chunk {64 d, kBN keys}, 64-byte rows
   constexpr int NS = kBN / 2;     // S accumulator registers per thread
   constexpr int NDC = kDS / 64;   // 64-column chunks of the slab
   constexpr uint32_t kPolyMask = kDS <= 64 ? B200_ATTN_POLY_MASK_D64 : (kDS <= 128 ? B200_ATTN_POLY_MASK : 0u);
@@ -206,12 +210,15 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t sq = smem_u32(smem);
   const uint32_t sring = sq + kWG * p.nq * 8192;
-  const uint32_t bars = sring + p.ring * SLOT;
+  const uint32_t sstg = sring + p.ring * SLOT;   // kFP8: the staging ring, one chunk per ring slot
+  const uint32_t bars = sstg + p.ring * STG;
   const uint32_t qbar = bars;
-  const uint32_t rowss = bars + 8u * (1 + 2 * p.ring);   // per-row sum of squares (fused RMS norm over slabs)
+  // per-row sum of squares (fused RMS norm over slabs)
+  const uint32_t rowss = bars + 8u * (1 + (kFP8 ? 3 : 2) * p.ring);
   const bool rms_cluster = p.rms_g > 0.f && p.slabs > 1;
   auto full = [&](int s) { return bars + 8u * (1 + s); };
   auto empty = [&](int s) { return bars + 8u * (1 + p.ring + s); };
+  [[maybe_unused]] auto staged = [&](int s) { return bars + 8u * (1 + 2 * p.ring + s); };   // kFP8: TMA landed
 
   const int wg = threadIdx.x / 128, tid = threadIdx.x % 128;
   // causal: the last query tile of a head has the most key blocks and starts first.  The head stays on grid.y, so the
@@ -250,17 +257,19 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
   // row of a sub-load comes from a page, so any partial key block is one.
   [[maybe_unused]] int vz = -1;
   [[maybe_unused]] const uint32_t vbar = rowss;   // its V chunks land here (no fused RMS norm with kSeqlens)
-  if constexpr (kSeqlens) {
+  // kFP8: the converters write those rows as zeros instead (vz stays -1)
+  if constexpr (kSeqlens && !kFP8) {
     if (p.Nk % kBN != 0 && (kPaged || p.Nk < nk_pad) && p.num_kv - 1 >= kv.x && p.num_kv - 1 < kv.y) vz = p.num_kv - 1;
   }
 
   if (threadIdx.x == 0) {
     mbar_init(qbar, 1);
     for (int s = 0; s < p.ring; ++s) {
-      mbar_init(full(s), 1);
+      mbar_init(full(s), kFP8 ? 3 : 1);   // kFP8: lane 0 of each converter warp
       mbar_init(empty(s), 4 * kWG);   // lane 0 of every consumer warp
+      if constexpr (kFP8) mbar_init(staged(s), 1);
     }
-    if constexpr (kSeqlens) mbar_init(vbar, 1);
+    if constexpr (kSeqlens && !kFP8) mbar_init(vbar, 1);
     fence_mbar_init();
   }
   __syncthreads();
@@ -298,17 +307,18 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
           for (int c = 0; c < p.nq + nvc; ++c, ++it) {
             const bool isv = c >= p.nq, zeroed = isv && j == vz;
             const int s = it % p.ring;
-            const uint32_t bar = zeroed ? vbar : full(s);
+            // kFP8: into the staging slot s, onto staged(s) (rows of R * 64 bytes)
+            const uint32_t bar = kFP8 ? staged(s) : (zeroed ? vbar : full(s));
             if (lane == 0) {
               if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
-              if (!zeroed) mbar_expect_tx(bar, KV_BYTES);
+              if (!zeroed) mbar_expect_tx(bar, kFP8 ? STG : KV_BYTES);
               else if (c == p.nq) mbar_expect_tx(vbar, nvc * KV_BYTES);
             }
             for (int i = 0; i < nsub; ++i) {
               const int r = __shfl_sync(0xffffffffu, cur, i);
               if (lane == 0)
-                tma_load_3d(sring + s * SLOT + i * R * 128, isv ? &tmap_v : &tmap_k, bar,
-                            isv ? d0 + 64 * (c - p.nq) : 64 * c, hk, r, kEvictLast);
+                tma_load_3d(kFP8 ? sstg + s * STG + i * R * 64 : sring + s * SLOT + i * R * 128,
+                            isv ? &tmap_v : &tmap_k, bar, isv ? d0 + 64 * (c - p.nq) : 64 * c, hk, r, kEvictLast);
             }
           }
         }
@@ -323,17 +333,20 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
         for (int c = 0; c < p.nq; ++c)
           tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, q0 + 64 * w, bh, kEvictFirst);
       int it = 0;
+      // kFP8: every K / V chunk goes to the staging slot s, onto staged(s)
+      auto landed = [&](int s) { return kFP8 ? staged(s) : full(s); };
+      auto dst = [&](int s) { return kFP8 ? sstg + s * STG : sring + s * SLOT; };
       auto next = [&](uint32_t bytes) {
         const int s = it % p.ring;
         if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
-        mbar_expect_tx(full(s), bytes);
+        mbar_expect_tx(landed(s), kFP8 ? STG : bytes);
         ++it;
         return s;
       };
       for (int j = kv.x; j < kv.y; ++j) {
         for (int c = 0; c < p.nq; ++c) {
           const int s = next(KV_BYTES);
-          tma_load_3d(sring + s * SLOT, &tmap_k, full(s), 64 * c, j * kBN, bh, kEvictLast);
+          tma_load_3d(dst(s), &tmap_k, landed(s), 64 * c, j * kBN, bh, kEvictLast);
         }
         for (int c = 0; c < nvc; ++c) {
           if constexpr (kVT) {
@@ -352,12 +365,48 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
               }
             }
             const int s = next(KV_BYTES);
-            tma_load_3d(sring + s * SLOT, &tmap_v, full(s), d0 + 64 * c, j * kBN, bh, kEvictLast);
+            tma_load_3d(dst(s), &tmap_v, landed(s), d0 + 64 * c, j * kBN, bh, kEvictLast);
           }
         }
       }
     }
-    if constexpr (kSeqlens) {
+    if constexpr (kFP8) {
+      if (tid >= 32) {
+        // warps 1-3 widen every staged chunk of the producer's order into its ring slot: 16 e4m3 bytes of staged row r
+        // (64 bytes per row) per thread and step, written as two 16-byte units of ring row r (128 bytes, 128B swizzle:
+        // unit u of row r at u ^ (r % 8)).  V rows of keys >= Lk_b are written as zeros (NaN bytes there must not
+        // reach P V); K rows past Lk_b are masked in the scores.
+        const int ct = tid - 32;
+        int it = 0;
+        for (int j = kv.x; j < kv.y; ++j) {
+          for (int c = 0; c < p.nq + nvc; ++c, ++it) {
+            const int s = it % p.ring;
+            const int rows = c >= p.nq ? min(kBN, p.Nk - j * kBN) : kBN;
+            mbar_wait(staged(s), (it / p.ring) & 1);
+            if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
+            const uint8_t* src = smem + (sstg - sq) + s * STG;
+            uint8_t* out = smem + (sring - sq) + s * SLOT;
+            for (int x = ct; x < kBN * 4; x += 96) {
+              const int r = x >> 2, q = x & 3;
+              uint4 lo = make_uint4(0u, 0u, 0u, 0u), hi = lo;
+              if (r < rows) {
+                const uint4 in = *reinterpret_cast<const uint4*>(src + 16 * x);
+                const uint2 a = e4m3x4_to<T>(in.x), b = e4m3x4_to<T>(in.y), d = e4m3x4_to<T>(in.z),
+                            e = e4m3x4_to<T>(in.w);
+                lo = make_uint4(a.x, a.y, b.x, b.y);
+                hi = make_uint4(d.x, d.y, e.x, e.y);
+              }
+              *reinterpret_cast<uint4*>(out + 128 * r + 16 * ((2 * q) ^ (r & 7))) = lo;
+              *reinterpret_cast<uint4*>(out + 128 * r + 16 * ((2 * q + 1) ^ (r & 7))) = hi;
+            }
+            fence_proxy_async_smem();   // the consumers' wgmma reads the slot through the async proxy
+            __syncwarp();
+            if (tid % 32 == 0) mbar_arrive(full(s));
+          }
+        }
+      }
+    }
+    if constexpr (kSeqlens && !kFP8) {
       if (tid / 32 == 1 && vz >= 0) {
         // a natural-V chunk {64 d, kBN keys} holds key r in the 128-byte row r (the 128B swizzle permutes 16-byte units
         // within a row only): zero rows Lk_b - vz * kBN .. kBN - 1 of the block's V chunks, then publish them
@@ -539,6 +588,11 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
   }
 
   // ---- epilogue
+  // kFP8: the normalised fp32 O times v_scale, then rounded once (kSplit: written to the workspace)
+  auto vs = [&](float x) {
+    if constexpr (kFP8) return x * v_scale;
+    else return x;
+  };
   const size_t head = static_cast<size_t>(bh) * p.Nq;
   float inv[2], lsum[2], ss[2];
 #pragma unroll
@@ -604,7 +658,8 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
             const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
             if (col < p.D)
               *reinterpret_cast<float2*>(orow + col) =
-                  make_float2(pad ? 0.f : o[c][4 * jj + 2 * i] * inv[i], pad ? 0.f : o[c][4 * jj + 2 * i + 1] * inv[i]);
+                  make_float2(pad ? 0.f : vs(o[c][4 * jj + 2 * i] * inv[i]),
+                              pad ? 0.f : vs(o[c][4 * jj + 2 * i + 1] * inv[i]));
           }
       }
       return;
@@ -639,7 +694,8 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
       for (int jj = 0; jj < 8; ++jj) {
         const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
         if (col < p.D)
-          *reinterpret_cast<uint32_t*>(orow + col) = pack(o[c][4 * jj + 2 * i] * inv[i], o[c][4 * jj + 2 * i + 1] * inv[i]);
+          *reinterpret_cast<uint32_t*>(orow + col) =
+              pack(vs(o[c][4 * jj + 2 * i] * inv[i]), vs(o[c][4 * jj + 2 * i + 1] * inv[i]));
       }
   }
 }
@@ -684,6 +740,36 @@ attn_fwd_paged_bf16_kernel(const __grid_constant__ CUtensorMap tmap_q, const __g
                            const Pages pages) {
   attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, kSplit, true, true, __nv_bfloat16>(tmap_q, tmap_k, tmap_v, p, lens,
                                                                                         pages);
+}
+
+// fp8 (e4m3) K and V with T = __half or __nv_bfloat16 Q and O (b200_fmha_fwd_{f16,bf16}_fp8kv_{seqlens,paged}): the two
+// kernels above, with K and V staged as e4m3 and widened exactly to T in shared memory.  The softmax scale arrives
+// with k_scale folded in; v_scale multiplies the normalised O.  Instantiated in attn_fp8kv_f16.cu / attn_fp8kv_bf16.cu.
+//   * the producer's lane 0 issues TMA loads of e4m3 chunks {64 d, kBN keys} (64-byte rows, no swizzle; paged: kBN / R
+//     sub-loads of R rows) into a staging ring of one chunk per ring slot, onto that chunk's `staged` barrier;
+//   * warps 1-3 of the producer warpgroup wait for the staged chunk and for the ring slot's `empty` barrier, widen
+//     the chunk with cvt.rn.f16x2.e4m3x2 (bf16: through fp32, also exact) into the 128B-swizzled layout the consumers
+//     read, fence the async proxy and arrive on the slot's `full` barrier (three arrivals);
+//   * the staging slot is free again once the ring slot is (its converters read it before publishing the slot), so
+//     the producer's wait on `empty` covers both;
+//   * V rows of keys >= Lk_b in the partial key block are written as zeros by the converters, which replaces warp 1's
+//     zeroing of the fp16 / bf16 kernels.
+template <int kDS, int kBN, int kWG, bool kCausal, bool kSplit, typename T>
+__global__ void __launch_bounds__(threads<kWG>(), 1)
+attn_fwd_fp8kv_seqlens_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                              const __grid_constant__ CUtensorMap tmap_v, const Params p, const Lens lens,
+                              const float v_scale) {
+  attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, kSplit, true, false, T, true>(tmap_q, tmap_k, tmap_v, p, lens,
+                                                                                  Pages{}, v_scale);
+}
+
+template <int kDS, int kBN, int kWG, bool kCausal, bool kSplit, typename T>
+__global__ void __launch_bounds__(threads<kWG>(), 1)
+attn_fwd_fp8kv_paged_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                            const __grid_constant__ CUtensorMap tmap_v, const Params p, const Lens lens,
+                            const Pages pages, const float v_scale) {
+  attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, kSplit, true, true, T, true>(tmap_q, tmap_k, tmap_v, p, lens,
+                                                                                 pages, v_scale);
 }
 
 }  // namespace attn

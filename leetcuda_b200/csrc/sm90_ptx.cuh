@@ -10,6 +10,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace b200 {
 
 #define B200_DEVICE __device__ __forceinline__
@@ -344,6 +346,28 @@ B200_DEVICE uint32_t pack_bf162(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
+}
+// four e4m3 values (bytes 0 .. 3 of x) widened to two f16x2 (.x: bytes 0, 1; .y: bytes 2, 3; the lower byte in the low
+// half).  Exact: every e4m3 value, subnormals and NaN included, is an fp16 value (F2FP.F16.E4M3.UNPACK_B on sm_90a).
+B200_DEVICE uint2 e4m3x4_to_half2x2(uint32_t x) {
+  uint2 r;
+  asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %2;\n\t"
+      "cvt.rn.f16x2.e4m3x2 %0, lo;\n\tcvt.rn.f16x2.e4m3x2 %1, hi;\n\t}"
+      : "=r"(r.x), "=r"(r.y)
+      : "r"(x));
+  return r;
+}
+// the same as bf16x2: through fp16 and fp32, both exact (an e4m3 value has 4 significant bits and an exponent inside
+// bf16's range), so every value, NaN included, keeps its value
+B200_DEVICE uint32_t half2_to_bf162(uint32_t h) {
+  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
+  return pack_bf162(f.x, f.y);
+}
+template <typename T>
+B200_DEVICE uint2 e4m3x4_to(uint32_t x) {
+  const uint2 h = e4m3x4_to_half2x2(x);
+  if constexpr (std::is_same_v<T, __nv_bfloat16>) return make_uint2(half2_to_bf162(h.x), half2_to_bf162(h.y));
+  else return h;
 }
 B200_DEVICE float fast_exp2(float x) {
   float y;

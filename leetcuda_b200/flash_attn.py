@@ -65,10 +65,12 @@ V_TRANSPOSED_OPS = {
 OP_NAMES = _BASIC + _ACC_F32 + _SWIZZLE + _OTHERS
 
 
-def _shapes(Q, K, V, O, v_transposed, same_length, grouped=False, dtype=torch.float16):
+def _shapes(Q, K, V, O, v_transposed, same_length, grouped=False, dtype=torch.float16, fp8=False):
     """(B, H, Nq, Nk, D, Hkv) of q, o [B,H,Nq,D], k [B,Hkv,Nk,D], v [B,Hkv,Nk,D] or [B,Hkv,D,Nk]; Nk = Nq if
-    same_length; Hkv = H unless grouped, where any Hkv dividing H is accepted."""
-    _check_dtype(Q, K, V, O, dtype)
+    same_length; Hkv = H unless grouped, where any Hkv dividing H is accepted.  fp8: the dtypes were checked by
+    _fp8_kv."""
+    if not fp8:
+        _check_dtype(Q, K, V, O, dtype)
     if Q.dim() != 4 or K.dim() != 4:
         raise RuntimeError("Tensor size mismatch!")
     B, H, Nq, D = Q.shape
@@ -99,6 +101,31 @@ def _element_type(Q, K, V, O):
     return torch.bfloat16
 
 
+_FP8_DTYPES = tuple(getattr(torch, n) for n in ("float8_e4m3fn", "float8_e5m2", "float8_e4m3fnuz", "float8_e5m2fnuz",
+                                                 "float8_e8m0fnu") if hasattr(torch, n))
+
+
+def _fp8_kv(Q, K, V, O):
+    """Q's dtype when K and V are float8_e4m3fn (the fp8-K/V call), None when neither is an fp8 tensor."""
+    dts = [t.dtype for t in (Q, K, V, O)]
+    if not any(d in _FP8_DTYPES for d in dts):
+        return None
+    names = ", ".join(str(d).replace("torch.", "") for d in dts)
+    if any(d in _FP8_DTYPES and d != torch.float8_e4m3fn for d in dts):
+        raise RuntimeError(f"leetcuda_b200.flash_attn: fp8 K/V must be float8_e4m3fn (float8_e5m2 and the other fp8 "
+                           f"formats are not supported), got Q, K, V, O = {names}")
+    if Q.dtype in _FP8_DTYPES or O.dtype in _FP8_DTYPES:
+        raise RuntimeError(f"leetcuda_b200.flash_attn: Q and O must be fp16 or bf16 (fp8 is for K and V only), "
+                           f"got Q, K, V, O = {names}")
+    if K.dtype != V.dtype:
+        raise RuntimeError(f"leetcuda_b200.flash_attn: K and V must share one dtype (both float8_e4m3fn), "
+                           f"got K {K.dtype}, V {V.dtype}".replace("torch.", ""))
+    if Q.dtype != O.dtype or Q.dtype not in (torch.float16, torch.bfloat16):
+        raise RuntimeError(f"leetcuda_b200.flash_attn: with fp8 K/V, Q and O must both be fp16 or both bf16, "
+                           f"got Q {Q.dtype}, O {O.dtype}".replace("torch.", ""))
+    return Q.dtype
+
+
 def _placement(*tensors):
     for t in tensors:
         if not t.is_cuda:
@@ -115,7 +142,8 @@ def _check(Q, K, V, O, v_transposed):
 
 
 def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=None, causal: bool = False,
-             num_splits: int = 1, seqlens_q=None, seqlens_k=None, block_table=None) -> None:
+             num_splits: int = 1, seqlens_q=None, seqlens_k=None, block_table=None, k_scale: float = 1.0,
+             v_scale: float = 1.0) -> None:
     """``O = softmax(Q K^T * scale) V`` on the current CUDA stream of ``Q``'s device.
 
     Q, O are ``[B,H,Nq,D]``; K is ``[B,Hkv,Nk,D]`` and V ``[B,Hkv,Nk,D]`` (or ``[B,Hkv,D,Nk]`` with ``v_transposed``),
@@ -152,7 +180,32 @@ def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=
     Q, K, V and O are all fp16 or all bf16 (``torch.bfloat16``: ``b200_fmha_fwd_bf16_seqlens`` / ``_paged``, every option
     above but ``v_transposed``; lse stays fp32).  A bf16 call rounds P and O to bf16 where an fp16 one rounds them to fp16
     and is otherwise the same computation; a bf16 call without lengths runs the per-sequence-length kernel with every
-    sequence at Nq / Nk."""
+    sequence at Nq / Nk.
+
+    K and V may also be ``torch.float8_e4m3fn`` (an fp8 KV cache, dense, per-sequence or paged) with Q and O both fp16
+    or both bf16 (``b200_fmha_fwd_{f16,bf16}_fp8kv_seqlens`` / ``_paged``): the call computes
+    ``softmax(scale * Q (k_scale * K)^T) (v_scale * V)`` with every option above but ``v_transposed``.  ``k_scale`` and
+    ``v_scale`` are per-tensor fp32 scales (finite, > 0; default 1) of the dequantisation ``x = scale * code``.  K and V
+    are widened exactly to Q's type on the GPU, k_scale is folded into the softmax scale (fp32(scale * k_scale)) and
+    v_scale multiplies the normalised O before its one rounding, so with v_scale = 1 the call is bit for bit the fp16 /
+    bf16 seqlens or paged call on ``K.to(Q.dtype)``, ``V.to(Q.dtype)`` with that folded scale.  Scales other than 1
+    are rejected with K and V that are not fp8."""
+    fp8 = _fp8_kv(Q, K, V, O)
+    if fp8 is not None:
+        if v_transposed:
+            raise RuntimeError("leetcuda_b200.flash_attn: transposed V is not supported with fp8 K/V "
+                               "(v_transposed=True with float8_e4m3fn tensors)")
+        scales = (float(k_scale), float(v_scale))
+        if block_table is not None:
+            _fmha_paged(Q, K, V, O, False, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table, fp8,
+                        scales)
+        else:
+            _fmha_seqlens(Q, K, V, O, False, scale, lse, causal, num_splits, seqlens_q, seqlens_k, fp8, scales)
+        return
+    if k_scale != 1.0 or v_scale != 1.0:
+        raise RuntimeError(f"leetcuda_b200.flash_attn: k_scale / v_scale apply to fp8 (float8_e4m3fn) K and V only, "
+                           f"got k_scale={k_scale!r}, v_scale={v_scale!r} with K {K.dtype}, V {V.dtype}"
+                           .replace("torch.", ""))
     dtype = _element_type(Q, K, V, O)
     if dtype == torch.bfloat16 and v_transposed:
         raise RuntimeError("leetcuda_b200.flash_attn: transposed V is fp16 only (v_transposed=True with bf16 tensors)")
@@ -173,18 +226,22 @@ def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=
 
 
 def _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k,
-                  dtype=torch.float16) -> None:
+                  dtype=torch.float16, fp8_scales=None) -> None:
     if v_transposed:
         raise RuntimeError("leetcuda_b200.flash_attn: seqlens_q / seqlens_k take natural V [B,Hkv,Nk,D] only "
                            "(v_transposed=True is not supported with lengths)")
-    B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, False, same_length=False, grouped=True, dtype=dtype)
+    B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, False, same_length=False, grouped=True, dtype=dtype,
+                                   fp8=fp8_scales is not None)
     _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k)
     _placement(Q, K, V, O, *(() if lse is None else (lse,)))
     args = [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), None if lse is None else lse.data_ptr(),
             None if seqlens_q is None else seqlens_q.data_ptr(), None if seqlens_k is None else seqlens_k.data_ptr(),
             B, H, Hkv, Nq, Nk, D, int(bool(causal)), int(num_splits), float(scale)]
-    fn = _capi.lib().b200_fmha_fwd_bf16_seqlens if dtype == torch.bfloat16 else _capi.lib().b200_fmha_fwd_f16_seqlens
-    _call_on_device(fn, args, Q.device.index)
+    name = "b200_fmha_fwd_bf16" if dtype == torch.bfloat16 else "b200_fmha_fwd_f16"
+    if fp8_scales is not None:
+        name += "_fp8kv"
+        args += list(fp8_scales)
+    _call_on_device(getattr(_capi.lib(), name + "_seqlens"), args, Q.device.index)
 
 
 def _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k) -> None:
@@ -204,11 +261,12 @@ def _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k) -> None:
 
 
 def _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table,
-                dtype=torch.float16) -> None:
+                dtype=torch.float16, fp8_scales=None) -> None:
     if v_transposed:
         raise RuntimeError("leetcuda_b200.flash_attn: block_table takes natural V pools [num_pages,page_size,Hkv,D] "
                            "only (v_transposed=True is not supported with a block table)")
-    _check_dtype(Q, K, V, O, dtype)
+    if fp8_scales is None:
+        _check_dtype(Q, K, V, O, dtype)
     if Q.dim() != 4 or tuple(O.shape) != tuple(Q.shape):
         raise RuntimeError("Tensor size mismatch!")
     B, H, Nq, D = Q.shape
@@ -231,8 +289,11 @@ def _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlen
             t.data_ptr(), None if seqlens_q is None else seqlens_q.data_ptr(),
             None if seqlens_k is None else seqlens_k.data_ptr(), B, H, Hkv, Nq, num_pages, page_size, t.shape[1], D,
             int(bool(causal)), int(num_splits), float(scale)]
-    fn = _capi.lib().b200_fmha_fwd_bf16_paged if dtype == torch.bfloat16 else _capi.lib().b200_fmha_fwd_f16_paged
-    _call_on_device(fn, args, Q.device.index)
+    name = "b200_fmha_fwd_bf16" if dtype == torch.bfloat16 else "b200_fmha_fwd_f16"
+    if fp8_scales is not None:
+        name += "_fp8kv"
+        args += list(fp8_scales)
+    _call_on_device(getattr(_capi.lib(), name + "_paged"), args, Q.device.index)
 
 
 def _call_on_device(fn, args, idx) -> None:

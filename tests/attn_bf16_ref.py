@@ -187,7 +187,8 @@ def online_split(q, k, v, scale, kbn, splits, poly_mask=0, part_round=None):
 
 # ------------------------------------------------------------------ the GPU case table
 # ("seqlens", attn_seqlens_ref's rows) and ("paged", attn_paged_ref's rows) reach every path key; the dense rows run the
-# seqlens kernel without lengths: MHA and GQA, causal or not, one split, several, or the library's choice (0).
+# seqlens kernel without lengths: MHA and GQA, causal or not, one split, several, or the library's choice (0), at
+# D = 40 .. 264 and at 1000 (four slabs, the smallest K/V ring: attn_ring_ref).
 Dense = namedtuple("Dense", "H Hkv Nq Nk D causal splits gens")
 DENSE = [
     Dense(4, 4, 257, 257, 64, False, 1, ("randn", "tail_max")),
@@ -196,9 +197,13 @@ DENSE = [
     Dense(8, 1, 1, 4100, 128, False, 0, ("randn", "front_max")),
     Dense(8, 2, 5, 777, 40, True, 3, ("randn", "diag_gather")),
     Dense(4, 2, 130, 300, 136, False, 2, ("randn", "one_hot")),
+    Dense(8, 2, 130, 330, 1000, True, 1, ("randn", "future_max")),
+    Dense(4, 1, 1, 1000, 1000, False, 4, ("randn", "tail_max")),
 ]
-CASES = ([("seqlens", c) for c in S.CASES_BY_SHAPE] + [("paged", c) for c in P.CASES_BY_SHAPE]
+_ROWS = ([("seqlens", c) for c in S.CASES_BY_SHAPE] + [("paged", c) for c in P.CASES_BY_SHAPE]
          + [("dense", c) for c in DENSE])
+# the rows of head dims > 512 (attn_ring_ref's regimes) last, so that the others keep their places
+CASES = [x for x in _ROWS if x[1].D <= 512] + [x for x in _ROWS if x[1].D > 512]
 
 
 def case_key(kind, c, splits=None):

@@ -98,14 +98,16 @@ def gather(pool, table, lk, Nk):
 # ------------------------------------------------------------------ the GPU case table
 # One row per path key.  Each row's sequences have the key lengths 0, 1, kBN - 1, kBN + 1, page_size - 1,
 # page_size + 1 and the full padded Nk, and query lengths that mix 0 or 1 with full ones; causal rows include Lq > Lk.
-# Shapes: D = 40 / 64 (kDS 64, kBN 128), 72 / 128 (kDS 128, kBN 64), 136 / 264 (kDS 256); G in {1, 4, 8}; Nq = 1 / 5
-# (decoding, packed tiles) and 130 (per-head tiles when causal).
+# Shapes: D = 40 / 64 (kDS 64, kBN 128), 72 / 128 (kDS 128, kBN 64), 136 / 264 and 520 / 776 / 1000 (kDS 256; three
+# and four slabs, from 776 on a K/V ring shorter than one key block); G in {1, 4, 8}; Nq = 1 / 5 (decoding, packed
+# tiles) and 130 (per-head tiles when causal).
 Case = namedtuple("Case", "H Hkv Nq page_size max_pages D causal splits lq lk gens")
 
 _FAMILIES = [   # (head dims, kBN, page sizes below / at / above kBN with the table width that gives Nk ~ 800)
     ((40, 64), 128, ((16, 50), (128, 6), (256, 3))),
     ((72, 128), 64, ((16, 50), (64, 12), (256, 3))),
     ((136, 264), 64, ((32, 25), (64, 12), (128, 6))),
+    ((520, 776, 1000), 64, ((16, 50), (64, 12), (256, 3))),   # a K/V ring shorter than one block (attn_ring_ref)
 ]
 # (causal, split, Nq): the six seqlens paths of a family (non-causal rows are packed whatever Nq)
 _PATHS = [(False, False, 1), (False, True, 130), (True, False, 5), (True, False, 130), (True, True, 5),
@@ -126,7 +128,7 @@ def _rows():
             for causal, split, Nq in _PATHS:
                 H, Hkv = _HEADS[n % 3]
                 gens = ("randn", (M.PROBES if causal else _ADVERSARIAL)[n % (2 if causal else 5)])
-                rows.append(Case(H, Hkv, Nq, ps, maxp, Ds[n % 2], causal, 2 + n % 5 if split else 1, _LQ[Nq],
+                rows.append(Case(H, Hkv, Nq, ps, maxp, Ds[n % len(Ds)], causal, 2 + n % 5 if split else 1, _LQ[Nq],
                                  _lk(kbn, ps, ps * maxp), gens))
                 n += 1
     return rows

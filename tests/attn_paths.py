@@ -90,7 +90,8 @@ def parse_instantiations(names):
 # One row per shape; every generator of the row is one case (attn_ref / attn_mask_ref generators).  The shapes reach
 # the edges of their kernel:
 #   D = 40 (a ragged 64-column slab), 72 (ragged 128), 136 (one ragged 256-column slab), 256 (one full slab), 264 (two
-#   slabs, the second 8 columns wide), 384 / 512 (the RMS cluster);
+#   slabs, the second 8 columns wide), 384 / 512 (the RMS cluster), 520 (three slabs, the last 8 columns wide), 776 /
+#   1000 (four slabs; the K/V ring holds less than one key block, at 1000 it is at its smallest: attn_ring_ref);
 #   Nk = 776 = 12 * 64 + 8 with V^T (Nk % 8 == 0 there): the last V^T box is 56 keys out of bounds, 777 / 300 / 1000
 #   ragged otherwise;
 #   Nq = 1 and 5 (packed decoding, speculative decoding), 130 (>= the tile rows: per-head tiles, a ragged last tile);
@@ -158,6 +159,14 @@ CASES_BY_SHAPE = [
     Case(2, 4, 4, 5, 776, 136, T, T, 4, F, ("randn", "ramp_max", "future_max")),
     Case(1, 2, 2, 136, 136, 136, T, F, 1, T, ("randn", "one_hot")),
     Case(1, 2, 2, 136, 136, 512, T, F, 1, T, ("randn", "neg_scores")),
+    # D = 520 / 776 / 1000: three slabs and four, a K/V ring shorter than one key block (776), the smallest ring
+    # (1000): attn_ring_ref.  Last in the table, so that the rows above keep their places.
+    Case(1, 8, 2, 130, 777, 776, F, T, 1, F, ("randn", "neg_scores", "future_max")),
+    Case(2, 8, 2, 5, 1000, 1000, F, T, 1, F, ("randn", "front_max", "diag_gather")),
+    Case(1, 8, 8, 130, 777, 1000, F, T, 5, F, ("randn", "ramp_max", "future_max")),
+    Case(1, 4, 1, 1, 1000, 776, F, F, 17, F, ("randn", "tail_max")),
+    Case(2, 4, 2, 130, 776, 1000, T, F, 1, F, ("randn", "one_hot")),
+    Case(1, 8, 2, 130, 776, 520, T, T, 3, F, ("randn", "tail_max", "diag_gather")),
 ]
 
 CASES = [(c, gen) for c in CASES_BY_SHAPE for gen in c.gens]

@@ -147,8 +147,10 @@ def part_references(q, k, v, scale, causal, splits, lq, lk, exact_scores=False):
 
 # ------------------------------------------------------------------ the GPU case table
 # Every row mixes the lengths of its sequences: Lk 0, 1, kBN - 1, kBN, kBN + 1, ragged and Nk; Lq 0, 1, 5 and Nq;
-# causal rows with Lq > Lk.  Shapes: D = 40 / 64 (kDS 64, kBN 128), 72 / 128 (kDS 128, kBN 64), 136 / 264 (kDS 256);
-# G in {1, 4, H}; Nq = 1 / 5 (decoding, packed tiles) and 130 (per-head tiles with Nq >= 128 rows, and Nq >= 64).
+# causal rows with Lq > Lk.  Shapes: D = 40 / 64 (kDS 64, kBN 128), 72 / 128 (kDS 128, kBN 64), 136 / 264 (kDS 256),
+# and 520 / 776 / 1000 (kDS 256: three slabs, the last one 8 columns, and four; from 776 on the K/V ring holds less
+# than one key block, at 1000 it is at its smallest); G in {1, 4, H}; Nq = 1 / 5 (decoding, packed tiles) and 130
+# (per-head tiles with Nq >= 128 rows, and Nq >= 64).
 Case = namedtuple("Case", "H Hkv Nq Nk D causal splits lq lk gens")
 F, T = False, True
 _LK128 = (0, 1, 127, 128, 129, 300, 777)
@@ -180,6 +182,13 @@ CASES_BY_SHAPE = [
     Case(4, 2, 130, 777, 136, T, 2, (130, 5, 1, 0, 130, 9, 64), _LK64, ("randn", "tail_max", "future_max")),
     Case(8, 8, 5, 777, 264, T, 3, (5, 0, 1, 5, 5, 5, 5), _LK64, ("randn", "front_max", "diag_gather")),
     Case(8, 8, 130, 300, 136, F, 3, (130, 1, 0, 5, 130, 70, 99), (0, 1, 63, 64, 65, 250, 300), ("randn", "one_hot")),
+    # head dims 520 / 776 / 1000: three slabs and four, a K/V ring shorter than one key block (attn_ring_ref)
+    Case(4, 4, 1, 777, 520, F, 1, (1, 1, 0, 1, 1, 1, 1), _LK64, ("randn", "tail_max")),
+    Case(8, 2, 5, 777, 776, T, 1, (5, 1, 5, 5, 0, 4, 5), _LK64, ("randn", "front_max", "diag_gather")),
+    Case(8, 2, 130, 777, 1000, T, 1, (130, 1, 5, 130, 0, 90, 129), _LK64, ("randn", "ramp_max", "future_max")),
+    Case(8, 1, 1, 777, 1000, F, 5, (1, 1, 1, 0, 1, 1, 1), _LK64, ("randn", "one_hot")),
+    Case(4, 2, 130, 777, 776, T, 2, (130, 5, 1, 0, 130, 9, 64), _LK64, ("randn", "neg_scores", "future_max")),
+    Case(8, 8, 5, 777, 520, T, 3, (5, 0, 1, 5, 5, 5, 5), _LK64, ("randn", "tail_max", "diag_gather")),
 ]
 
 CASES = [(c, gen) for c in CASES_BY_SHAPE for gen in c.gens]

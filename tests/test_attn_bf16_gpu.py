@@ -37,7 +37,7 @@ from leetcuda_b200 import _capi, flash_attn
 from leetcuda_b200 import merge_attn_states as MA
 from test_attn_gqa_gpu import _inputs
 from test_attn_numerics_gpu import MARGIN, SENT32, _assert_margins
-from test_attn_seqlens_gpu import _kernels, _lens, _poison
+from test_attn_seqlens_gpu import _kernels_per_call, _lens, _poison
 
 pytestmark = pytest.mark.gpu
 
@@ -410,8 +410,8 @@ def test_sdpa_bf16():
 # ------------------------------------------------------------------ kernel names
 # torch.profiler runs in a child process.  In one process, a profiler session followed by many launches leaves later
 # sessions without CUDA records (see test_attn_paged_gpu.test_kernel_names), and this module runs before the fp16
-# modules whose kernel-name tests rely on being the first sessions of the process.  The child runs one session per case,
-# one right after another, and reports the names; the parent process never starts the profiler.
+# modules whose kernel-name tests rely on being the first sessions of the process.  The child runs every case in one
+# session (test_attn_seqlens_gpu._kernels_per_call) and reports the names; the parent process never starts the profiler.
 def _case_call(i):
     """(path key, a call of case i on fresh randn inputs, description)."""
     kind, c = BF.CASES[i]
@@ -438,11 +438,8 @@ def _case_call(i):
 
 def _profile_all_cases():
     """Child process: the CUDA kernel names of every case under torch.profiler, as one JSON line on stdout."""
-    out = []
-    for i in range(len(BF.CASES)):
-        _, fn, _ = _case_call(i)
-        out.append(_kernels(fn))
-    print("KERNEL_NAMES " + json.dumps(out))
+    fns = [_case_call(i)[1] for i in range(len(BF.CASES))]
+    print("KERNEL_NAMES " + json.dumps(_kernels_per_call(fns)))
 
 
 @pytest.fixture(scope="module")

@@ -35,7 +35,7 @@ import attn_split_ref as SR
 from leetcuda_b200 import _capi, flash_attn
 from test_attn_gqa_gpu import _inputs
 from test_attn_numerics_gpu import MARGIN, SENT32, _assert_margins
-from test_attn_seqlens_gpu import _kernels, _lens
+from test_attn_seqlens_gpu import _kernels_per_call, _lens
 
 pytestmark = pytest.mark.gpu
 
@@ -400,7 +400,7 @@ def test_benchmarked_shape(index, T):
 
 
 # ------------------------------------------------------------------ kernel names
-# torch.profiler runs in a child process, one session per case; the test process never starts the profiler (see
+# torch.profiler runs in a child process, all cases in one session; the test process never starts the profiler (see
 # test_attn_bf16_gpu: a session followed by many launches leaves later sessions of the process without CUDA records).
 def _case_call(i):
     T, kind, c = F.CASES[i]
@@ -424,11 +424,8 @@ def _case_call(i):
 
 def _profile_all_cases():
     """Child process: the CUDA kernel names of every case under torch.profiler, as one JSON line on stdout."""
-    out = []
-    for i in range(len(F.CASES)):
-        _, fn, _ = _case_call(i)
-        out.append(_kernels(fn))
-    print("KERNEL_NAMES " + json.dumps(out))
+    fns = [_case_call(i)[1] for i in range(len(F.CASES))]
+    print("KERNEL_NAMES " + json.dumps(_kernels_per_call(fns)))
 
 
 @pytest.fixture(scope="module")

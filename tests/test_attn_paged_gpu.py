@@ -10,8 +10,8 @@ table entries past each sequence's pages are -1, INT_MIN or ids of poisoned page
   * the fp64 reference with each sequence's visibility (attn_seqlens_ref.reference / part_references,
     attn_split_ref.combine_bound when split); padded rows and rows without a key exactly O = 0, lse = -inf; the pool
     and the table come back unchanged;
-  * _capi.launch_count() up by 1 unsplit, 2 split; under torch.profiler the restated attn_fwd_paged_kernel<...>, the
-    combine exactly when it splits.
+  * _capi.launch_count() up by 1 unsplit, 2 split; under torch.profiler (in a child process) the restated
+    attn_fwd_paged_kernel<...>, the combine exactly when it splits.
 Then pages shared between sequences, a 65536-key sequence in 16-key pages among short ones, CUDA graphs replayed with
 new tables and lengths, a side stream, every shape of tools/bench_attn_paged.py at full size, and SDPA with an
 explicit mask.  The largest |err| / bound per path is printed at the end of the module (pytest -s).
@@ -33,7 +33,7 @@ import attn_split_ref as SR
 from leetcuda_b200 import _capi, flash_attn
 from test_attn_gqa_gpu import _inputs
 from test_attn_numerics_gpu import _assert_margins, _guarded
-from test_attn_seqlens_gpu import _kernels, _lens, _poison
+from test_attn_seqlens_gpu import _kernels_per_call, _lens, _poison, profiled_names_of
 
 pytestmark = pytest.mark.gpu
 
@@ -321,20 +321,33 @@ def test_sdpa_with_an_explicit_mask():
 
 
 # ------------------------------------------------------------------ kernel names
-# Last in the module, one profiler session right after another.  On an H100, in one process, torch.profiler sessions
-# that came after an earlier session followed by the many launches of the tests above recorded no CUDA kernel at all,
-# here and in the modules that follow (test_attn_paths_gpu, test_attn_seqlens_gpu).
+# torch.profiler runs in a child process, all cases in one session (test_attn_seqlens_gpu._kernels_per_call); this
+# process never starts it.  On an H100, in one process, sessions that came after an earlier session followed by many
+# launches recorded some or none of their kernels.
+def _profile_all_cases():
+    """Child process: the CUDA kernel names of every case, as one JSON line on stdout."""
+    import json
+    fns = []
+    for i, c in enumerate(P.CASES_BY_SHAPE):
+        q, k, v = _inputs("randn", len(c.lq), c.H, c.Hkv, c.Nq, c.page_size * c.max_pages, c.D, None, seed=i)
+        kp, vp, table = paginate(k, v, c.lk, c.page_size, c.max_pages, 0.0, seed=i)
+        lq, lk, o = _lens(c.lq), _lens(c.lk), torch.empty_like(q)
+        fns.append(lambda a=(q, kp, vp, table, o, None, c.causal, c.splits, lq, lk): _call(*a))
+    print("KERNEL_NAMES " + json.dumps(_kernels_per_call(fns)))
+
+
+@pytest.fixture(scope="module")
+def profiled_names():
+    return profiled_names_of("test_attn_paged_gpu")
+
+
 @pytest.mark.parametrize("i", range(len(P.CASES_BY_SHAPE)),
                          ids=lambda i: f"case{i}-D{P.CASES_BY_SHAPE[i].D}-page{P.CASES_BY_SHAPE[i].page_size}")
-def test_kernel_names(i):
+def test_kernel_names(profiled_names, i):
     c = P.CASES_BY_SHAPE[i]
-    B, Nk = len(c.lq), c.page_size * c.max_pages
-    key, _ = P.path(B, c.H, c.Hkv, c.Nq, c.page_size, c.max_pages, c.D, c.causal, c.splits)
-    q, k, v = _inputs("randn", B, c.H, c.Hkv, c.Nq, Nk, c.D, None, seed=i)
-    kp, vp, table = paginate(k, v, c.lk, c.page_size, c.max_pages, 0.0, seed=i)
-    lq, lk, o = _lens(c.lq), _lens(c.lk), torch.empty_like(q)
+    key, _ = P.path(len(c.lq), c.H, c.Hkv, c.Nq, c.page_size, c.max_pages, c.D, c.causal, c.splits)
     what = f"{label(key)}: H{c.H} Hkv{c.Hkv} Nq{c.Nq} page{c.page_size}x{c.max_pages} D{c.D} splits={c.splits}"
-    names = _kernels(lambda: _call(q, kp, vp, table, o, None, c.causal, c.splits, lq, lk))
+    names = profiled_names[i] if i < len(profiled_names) else []
     assert names, what + ": the profiler recorded no kernel"
     assert P.parse_instantiations(names) == [P.instantiation(key)], f"{what}: ran {names}"
     assert not S.parse_instantiations(names), f"{what}: ran {names}"

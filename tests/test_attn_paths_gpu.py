@@ -8,17 +8,15 @@ Each case of attn_paths.CASES is checked the way the sibling modules check their
     with the fused RMS norm); split: attn_split_ref.combine_bound; rows without a key exactly O = 0, lse = -inf;
   * GQA without a split bit for bit the same call on the expanded K/V; every non-RMS case again with lse=None, O bit
     for bit the same; _capi.launch_count() up by exactly the launches attn_paths.path restates;
-  * the path itself on the device: under torch.profiler the recorded attn_fwd_kernel<...> is the restated
-    instantiation, the transpose pre-pass runs exactly when the path has it, the combine exactly when it splits.
+  * the path itself on the device: under torch.profiler (in a child process) the recorded attn_fwd_kernel<...> is the
+    restated instantiation, the transpose pre-pass runs exactly when the path has it, the combine exactly when it splits.
 The largest |err| / bound per path is printed at the end of the module (pytest -s).
 """
 import collections
 import math
-import time
 
 import pytest
 import torch
-from torch.profiler import ProfilerActivity, profile
 
 import attn_mask_ref as M
 import attn_paths as P
@@ -27,11 +25,11 @@ import attn_split_ref as SR
 from leetcuda_b200 import _capi, flash_attn, fused_ops
 from test_attn_gqa_gpu import _inputs
 from test_attn_numerics_gpu import RMS_G, _assert_margins, _guarded
+from test_attn_seqlens_gpu import _kernels_per_call, profiled_names_of
 
 pytestmark = pytest.mark.gpu
 
 _ratios = collections.defaultdict(float)
-_empty_sessions = 0
 
 
 def label(key):
@@ -48,7 +46,6 @@ def _report():
               "attn_split_ref.combine_bound):")
         for key in sorted({k for k, _ in _ratios}):
             print(f"  {label(key):<48} O {_ratios[(key, 'O')]:.3f}  lse {_ratios[(key, 'lse')]:.3f}")
-        print(f"profiler sessions without a CUDA record, repeated: {_empty_sessions}")
 
 
 def _call(c, q, k, varg, o, lse):
@@ -70,25 +67,6 @@ def _run(c, q, k, varg):
     _assert_margins(obuf, "O")
     _assert_margins(lbuf, "lse")
     return o, lse, launches
-
-
-def _kernels(fn):
-    """Names of the CUDA kernels fn launches, recorded by torch.profiler.  Now and then a session comes back without
-    any CUDA record (two sessions in a row out of ~130 on an H100); such a session is repeated, at most twice, and
-    counted in the report.  The kernels run a few ms inside the session, away from the edges of its window."""
-    global _empty_sessions
-    for _ in range(3):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            time.sleep(0.002)
-            fn()
-            torch.cuda.synchronize()
-            time.sleep(0.002)
-        names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-        if names:
-            return names
-        _empty_sessions += 1
-    return []
 
 
 def _check(key, got, want, bound, empty, what):
@@ -141,11 +119,36 @@ def test_path_against_fp64(i):
             torch.cuda.synchronize()
             assert torch.equal(o, o2), what + ": O with lse=None differs"
 
-        names = _kernels(lambda: _call(c, q, k, varg, torch.empty_like(o), torch.empty_like(lse)))
-        assert names, what + ": the profiler recorded no kernel"
-        assert P.parse_instantiations(names) == [P.instantiation(key)], f"{what}: ran {names}"
-        assert sum("transpose_dn_to_nd_kernel" in s for s in names) == int(key[7]), f"{what}: ran {names}"
-        assert sum("attn_combine_kernel" in s for s in names) == int(key[6]), f"{what}: ran {names}"
+
+# torch.profiler runs in a child process, all cases in one session (test_attn_seqlens_gpu._kernels_per_call); this
+# process never starts it.
+def _profile_all_cases():
+    """Child process: the CUDA kernel names of every case, as one JSON line on stdout."""
+    import json
+    fns = []
+    for i, c in enumerate(P.CASES_BY_SHAPE):
+        q, k, v = _inputs("randn", c.B, c.H, c.Hkv, c.Nq, c.Nk, c.D, None, seed=i)
+        varg = v.transpose(-2, -1).contiguous() if c.vt else v
+        o, lse = torch.empty_like(q), torch.empty(q.shape[:3], device="cuda")
+        fns.append(lambda a=(c, q, k, varg, o, lse): _call(*a))
+    print("KERNEL_NAMES " + json.dumps(_kernels_per_call(fns)))
+
+
+@pytest.fixture(scope="module")
+def profiled_names():
+    return profiled_names_of("test_attn_paths_gpu")
+
+
+@pytest.mark.parametrize("i", range(len(P.CASES_BY_SHAPE)), ids=lambda i: f"case{i}-D{P.CASES_BY_SHAPE[i].D}")
+def test_kernel_names(profiled_names, i):
+    c = P.CASES_BY_SHAPE[i]
+    key, _ = P.path(c.B, c.H, c.Hkv, c.Nq, c.Nk, c.D, c.vt, c.causal, c.splits, c.rms)
+    what = f"{label(key)}: B{c.B} H{c.H} Hkv{c.Hkv} Nq{c.Nq} Nk{c.Nk} D{c.D} splits={c.splits}"
+    names = profiled_names[i] if i < len(profiled_names) else []
+    assert names, what + ": the profiler recorded no kernel"
+    assert P.parse_instantiations(names) == [P.instantiation(key)], f"{what}: ran {names}"
+    assert sum("transpose_dn_to_nd_kernel" in s for s in names) == int(key[7]), f"{what}: ran {names}"
+    assert sum("attn_combine_kernel" in s for s in names) == int(key[6]), f"{what}: ran {names}"
 
 
 # ------------------------------------------------------------------ workspaces under streams and graphs

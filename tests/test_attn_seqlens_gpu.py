@@ -8,8 +8,8 @@ or 65504 (in turn over the generators), Q rows >= Lq_b hold NaN, and O / lse sit
     lse = -inf; the inputs come back unchanged;
   * unsplit: every sequence's rows bit for bit fmha_fwd on that sequence alone (Nq = Lq_b, Nk = Lk_b);
   * full-length arrays: bit for bit the call without lengths, split or not;
-  * _capi.launch_count() up by 1 unsplit, 2 split; under torch.profiler the restated attn_fwd_seqlens_kernel<...>,
-    the combine exactly when it splits.
+  * _capi.launch_count() up by 1 unsplit, 2 split; under torch.profiler (in a child process) the restated
+    attn_fwd_seqlens_kernel<...>, the combine exactly when it splits.
 Then clamping, CUDA graphs and a side stream, a 65536-key sequence among short ones, and SDPA with an explicit mask.
 The largest |err| / bound per path is printed at the end of the module (pytest -s).
 """
@@ -84,20 +84,64 @@ def _poison(q, k, v, lq, lk, value):
     return q, k, v
 
 
-def _kernels(fn):
-    """Names of the CUDA kernels fn launches (torch.profiler); a session without a CUDA record is repeated, as in
-    test_attn_paths_gpu."""
+def _kernels_per_call(fns):
+    """[names of the CUDA kernels fn launches for fn in fns] from one torch.profiler session.  On an H100, a process that
+    had run some 30 short sessions recorded later ones without some or all of their kernels; a single session for all calls
+    does not depend on that.  The calls run one after another on a synchronised device, and the records split at a
+    marker kernel (torch.cuda._sleep) launched before every call and after the last."""
+    out = []
     for _ in range(3):
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             time.sleep(0.002)
-            fn()
+            for fn in fns:
+                torch.cuda._sleep(1)
+                fn()
+                torch.cuda.synchronize()
+            torch.cuda._sleep(1)
             torch.cuda.synchronize()
             time.sleep(0.002)
-        names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-        if names:
-            return names
-    return []
+        names = [e.name for e in sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA),
+                                        key=lambda e: e.time_range.start)]
+        out = []
+        for name in names:
+            if name == names[0]:
+                out.append([])
+            else:
+                out[-1].append(name)
+        out = out[:-1]
+        if len(out) == len(fns) and names.count(names[0]) == len(fns) + 1:
+            return out
+    return out
+
+
+def _profile_all_cases():
+    """Child process: the CUDA kernel names of every case, as one JSON line on stdout."""
+    import json
+    fns = []
+    for i, c in enumerate(S.CASES_BY_SHAPE):
+        q, k, v = _inputs("randn", len(c.lq), c.H, c.Hkv, c.Nq, c.Nk, c.D, None, seed=i)
+        lq, lk, o = _lens(c.lq), _lens(c.lk), torch.empty_like(q)
+        fns.append(lambda q=q, k=k, v=v, o=o, c=c, lq=lq, lk=lk: _call(q, k, v, o, None, c.causal, c.splits, lq, lk))
+    print("KERNEL_NAMES " + json.dumps(_kernels_per_call(fns)))
+
+
+def profiled_names_of(module):
+    """Run module._profile_all_cases() in a child process and return what it reports."""
+    import json
+    import os
+    import subprocess
+    import sys
+    from pathlib import Path
+    tests = Path(__file__).resolve().parent
+    env = dict(os.environ, PYTHONPATH=os.pathsep.join([str(tests.parent), str(tests)]
+                                                      + [p for p in [os.environ.get("PYTHONPATH")] if p]))
+    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
+        "-c", f"import {module} as T; T._profile_all_cases()"]
+    r = subprocess.run(cmd, cwd=tests.parent, env=env, capture_output=True, text=True, timeout=900)
+    lines = [x for x in r.stdout.splitlines() if x.startswith("KERNEL_NAMES ")]
+    assert r.returncode == 0 and lines, f"profiling child failed ({r.returncode}):\n{r.stdout[-2000:]}{r.stderr[-4000:]}"
+    return json.loads(lines[-1][len("KERNEL_NAMES "):])
 
 
 def _check(key, got, want, bound, empty, what):
@@ -160,11 +204,25 @@ def test_case_against_fp64(i):
             flash_attn.fmha_fwd(q0, k0, v0, go, lse=gl, causal=c.causal, num_splits=c.splits)
             torch.cuda.synchronize()
             assert torch.equal(fo, go) and torch.equal(fl, gl), what + ": full lengths differ from the call without"
-            names = _kernels(lambda: _call(q, k, v, torch.empty_like(o), None, c.causal, c.splits, lq, lk))
-            assert names, what + ": the profiler recorded no kernel"
-            assert S.parse_instantiations(names) == [S.instantiation(key)], f"{what}: ran {names}"
-            assert not any("attn_fwd_kernel<" in s for s in names), f"{what}: ran {names}"
-            assert sum("attn_combine_kernel" in s for s in names) == int(key[4]), f"{what}: ran {names}"
+
+
+# torch.profiler runs in a child process, all cases in one session; this process never starts it (see
+# _kernels_per_call, and test_attn_bf16_gpu: the fp16 modules that sort after this one rely on the first sessions).
+@pytest.fixture(scope="module")
+def profiled_names():
+    return profiled_names_of("test_attn_seqlens_gpu")
+
+
+@pytest.mark.parametrize("i", range(len(S.CASES_BY_SHAPE)), ids=lambda i: f"case{i}-D{S.CASES_BY_SHAPE[i].D}")
+def test_kernel_names(profiled_names, i):
+    c = S.CASES_BY_SHAPE[i]
+    key, _ = S.path(len(c.lq), c.H, c.Hkv, c.Nq, c.Nk, c.D, c.causal, c.splits)
+    what = f"{label(key)}: H{c.H} Hkv{c.Hkv} Nq{c.Nq} Nk{c.Nk} D{c.D} splits={c.splits}"
+    names = profiled_names[i] if i < len(profiled_names) else []
+    assert names, what + ": the profiler recorded no kernel"
+    assert S.parse_instantiations(names) == [S.instantiation(key)], f"{what}: ran {names}"
+    assert not any("attn_fwd_kernel<" in s for s in names), f"{what}: ran {names}"
+    assert sum("attn_combine_kernel" in s for s in names) == int(key[4]), f"{what}: ran {names}"
 
 
 @pytest.mark.parametrize("splits", [1, 3])

@@ -262,6 +262,54 @@ int b200_fmha_fwd_bf16_paged(const void* q, const void* k_cache, const void* v_c
                              int H, int Hkv, int Nq, int num_pages, int page_size, int max_pages_per_seq, int D,
                              int causal, int num_splits, float scale, void* stream);
 
+/* Packed variable-length attention (FlashAttention's flash_attn_varlen_func layout): the tokens of B sequences packed
+ * one after the other, no padding.
+ *
+ * q, o: [total_q, H, D].  k, v: [total_k, Hkv, D].  lse: fp32 [H, total_q] or NULL (the layout of
+ * b200_merge_attn_states' lse).  cu_seqlens_q, cu_seqlens_k: int32 [B + 1] in device memory.  Sequence b has
+ * Lq_b = clamp(cu_seqlens_q[b+1] - cu_seqlens_q[b], 0, max_seqlen_q) queries at rows cu_seqlens_q[b] + t and
+ * Lk_b = clamp(cu_seqlens_k[b+1] - cu_seqlens_k[b], 0, max_seqlen_k) keys at rows cu_seqlens_k[b] + t.  Query head h
+ * reads K/V head h / (H / Hkv).  Causal masking is per sequence and bottom-right: key j is masked for query i when
+ * j > i + (Lk_b - Lq_b); a row without a visible key (Lk_b = 0 included) gets O = 0 and lse = -inf.
+ * Only rows cu_seqlens_q[b] + t with t < Lq_b and 0 <= cu_seqlens_q[b] + t < total_q are written: rows of o and
+ * columns of lse that no sequence owns keep their contents, whatever the arrays hold (bad offsets give wrong values,
+ * never an out-of-bounds store; loads are bounds-checked TMA coordinates).  Keys of the next sequence in the last
+ * partial key block of sequence b contribute nothing, whatever they hold.  The offsets are read by the kernel only
+ * (no host copy, no synchronisation), so a captured CUDA graph replays with new offsets written into the same arrays.
+ * Numerics: O and lse are those of b200_fmha_fwd_f16_seqlens with num_splits = 1 on padded [B,H,max_seqlen_q,D] /
+ * [B,Hkv,max_seqlen_k,D] copies of the same data, bit for bit.  One launch, no workspace, no split.
+ * Every query head gets ceil(max_seqlen_q / 128) tiles of its own (of 64 rows for D > 128): a batch of one-token
+ * decode rows runs at 1/128 of the tile's rows; decoding should use the seqlens or paged entries.
+ * Constraints: B, H, D, total_q, total_k, max_seqlen_q, max_seqlen_k >= 1; Hkv >= 1 divides H; B * Hkv <= 65535;
+ * (H / Hkv) * max_seqlen_q <= 2^31 - 1 and the grid's (H / Hkv) * ceil(max_seqlen_q / 128) * slabs CTAs as well;
+ * total_q * H * D and total_k * Hkv * D addressable; the offset arrays 4-byte aligned; D % 8 == 0 and D <= 1024
+ * (B200_ENOTSUP otherwise).  scale <= 0 means 1/sqrt(D).  bf16: the same entry with bf16 q, k, v and o. */
+int b200_fmha_fwd_f16_varlen(const void* q, const void* k, const void* v, void* o, float* lse /* may be NULL */,
+                             const int* cu_seqlens_q, const int* cu_seqlens_k, int B, int H, int Hkv, int total_q,
+                             int total_k, int max_seqlen_q, int max_seqlen_k, int D, int causal, float scale,
+                             void* stream);
+int b200_fmha_fwd_bf16_varlen(const void* q, const void* k, const void* v, void* o, float* lse /* may be NULL */,
+                              const int* cu_seqlens_q, const int* cu_seqlens_k, int B, int H, int Hkv, int total_q,
+                              int total_k, int max_seqlen_q, int max_seqlen_k, int D, int causal, float scale,
+                              void* stream);
+
+/* Packed queries against a paged KV cache (vLLM's chunked prefill): b200_fmha_fwd_f16_varlen with k_cache, v_cache
+ * pools [num_pages, page_size, Hkv, D] and block_table int32 [B, max_pages_per_seq] as in b200_fmha_fwd_f16_paged.
+ * Sequence b has Lk_b = clamp(seqused_k[b], 0, max_pages_per_seq * page_size) keys (seqused_k: int32 [B] in device
+ * memory); key t is row t % page_size of page block_table[b][t / page_size].  Every other rule is the packed rule.
+ * Numerics: bit for bit b200_fmha_fwd_f16_paged with num_splits = 1 on a padded copy of q.  Constraints: those of the
+ * packed entry without total_k / max_seqlen_k, and the paged constraints of b200_fmha_fwd_f16_paged. */
+int b200_fmha_fwd_f16_varlen_paged(const void* q, const void* k_cache, const void* v_cache, void* o,
+                                   float* lse /* may be NULL */, const int* cu_seqlens_q, const int* seqused_k,
+                                   const int* block_table, int B, int H, int Hkv, int total_q, int max_seqlen_q,
+                                   int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
+                                   float scale, void* stream);
+int b200_fmha_fwd_bf16_varlen_paged(const void* q, const void* k_cache, const void* v_cache, void* o,
+                                    float* lse /* may be NULL */, const int* cu_seqlens_q, const int* seqused_k,
+                                    const int* block_table, int B, int H, int Hkv, int total_q, int max_seqlen_q,
+                                    int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
+                                    float scale, void* stream);
+
 /* ------------------------------------------------------------------ SGEMM (TF32)
  * C[M,N] (fp32) = A[M,K] (fp32) x B on the tensor cores through wgmma .tf32 with fp32
  * accumulation — the sibling of the HGEMM path (SURVEY §8f-2).  Replaces

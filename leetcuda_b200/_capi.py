@@ -55,7 +55,13 @@ SIGNATURES = {
                                            _i, _f, _f, _f, _vp]),
     "b200_fmha_fwd_bf16_fp8kv_paged": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i,
                                             _i, _f, _f, _f, _vp]),
-    "b200_fmha_fwd_f16_rmsnorm": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
+    "b200_fmha_fwd_f16_varlen": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _vp]),
+    "b200_fmha_fwd_bf16_varlen": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _vp]),
+    "b200_fmha_fwd_f16_varlen_paged": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i,
+                                            _i, _f, _vp]),
+    "b200_fmha_fwd_bf16_varlen_paged": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i,
+                                             _i, _f, _vp]),
+    "b200_fmha_fwd_f16_rmsnorm":(_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
     "b200_rope_f32": (_i, [_vp, _vp, _i, _i, _vp]),
     "b200_rope_qk_f16": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200_rms_norm": (_i, [_vp, _vp, _f, _i, _i, _i, _vp]),

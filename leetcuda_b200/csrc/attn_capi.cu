@@ -158,6 +158,30 @@ Family family(int D) {
   return {ds, ds == 64 ? 128 : 64, ds == 256 ? 1 : 2};
 }
 
+// The K/V ring of family f next to Q (nq 64-column chunks per tile row): every slot that fits, at most 16 (two key
+// blocks of K and V chunks at D = 512).  stage: the bytes each slot adds beside it (fp8: its staging chunk and
+// barrier).  Returns the dynamic shared memory with *ring slots, or 0 when fewer than two fit.
+int ring_smem(const Family& f, int nq, bool vt, int stage, int* ring) {
+  const int kMaxSmem = 227 * 1024;
+  const int slot = attn::slot_bytes(f.bn, f.ds, vt);
+  const int fixed = attn::smem_bytes(f.wgs, slot, nq, 0);
+  *ring = (kMaxSmem - fixed) / (slot + 16 + stage);
+  if (*ring > 16) *ring = 16;
+  if (*ring < 2) return 0;
+  return attn::smem_bytes(f.wgs, slot, nq, *ring) + *ring * stage;
+}
+
+// A tensor map over `rows` rows of `heads` heads of D elements (row-major [rows, heads, D]): dims {D, heads, rows},
+// boxes of {64, 1, box_rows}, 128B-swizzled unless given.  The paged pools [num_pages * page_size, Hkv, D] and the
+// token-major varlen Q [total_q, H, D] and K / V [total_k, Hkv, D].
+int rows_map(CUtensorMap* m, const void* base, int D, int heads, uint64_t rows, int box_rows, uint64_t elem_bytes,
+             CUtensorMapDataType dt, CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B) {
+  uint64_t dims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(heads), rows};
+  uint64_t str[2] = {static_cast<uint64_t>(D) * elem_bytes, static_cast<uint64_t>(heads) * D * elem_bytes};
+  uint32_t box[3] = {64, 1, static_cast<uint32_t>(box_rows)};
+  return host::get_tmap(m, base, 3, dims, str, box, sw, dt);
+}
+
 // G: query heads per K/V head (H = G * Hkv; the kernel sees B * Hkv heads of G * Nq packed rows).  splits > 1: grid.z
 // splits whose fp32 parts go to ws_o / ws_lse instead of o / lse (kSplit kernels).  Causal with G > 1 runs kGQA.
 // pages: k and v are pools of num_pages pages [page_size, Hkv, D], and Nk is the padded max_pages * page_size.
@@ -191,16 +215,9 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
   p.ws_lse = splits > 1 ? ws_lse : nullptr;
   if (rms_g > 0.f && D > 256 && !(D <= 512 && D % 128 == 0))
     return fail(B200_ENOTSUP, "fused rms_norm: D=%d (supported: D <= 256, 384, 512)", D);
-  // ring: every slot that fits next to Q, at most 16 (two key blocks of K and V chunks at D = 512)
-  const int kMaxSmem = 227 * 1024;
-  const int slot = attn::slot_bytes(bn, ds, vt);
-  const int fixed = attn::smem_bytes(wgs, slot, p.nq, 0);
   // fp8: every ring slot has a staging chunk of e4m3 bytes and its barrier beside it (attn_sm90.cuh)
-  const int stage = fp8 ? 64 * bn + 8 : 0;
-  p.ring = (kMaxSmem - fixed) / (slot + 16 + stage);
-  if (p.ring > 16) p.ring = 16;
-  if (p.ring < 2) return fail(B200_ENOTSUP, "headdim not support! (D=%d)", D);
-  const int smem = attn::smem_bytes(wgs, slot, p.nq, p.ring) + p.ring * stage;
+  const int smem = ring_smem(f, p.nq, vt, fp8 ? 64 * bn + 8 : 0, &p.ring);
+  if (smem == 0) return fail(B200_ENOTSUP, "headdim not support! (D=%d)", D);
   // causal packed heads of at least one tile of rows: tiles of their own per head (attn_sm90.cuh), else packed tiles
   p.tph = causal && Nq >= 64 * wgs ? (Nq + 64 * wgs - 1) / (64 * wgs) : 0;
   const int qtiles = p.tph > 0 ? G * p.tph : (rows + 64 * wgs - 1) / (64 * wgs);
@@ -222,12 +239,10 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
   if ((rc = host::get_tmap(&tq, q, 3, qdims, qstr, qbox, CU_TENSOR_MAP_SWIZZLE_128B, dt))) return rc;
   if (pages) {
     // pool rows {D, Hkv, num_pages * page_size}; a key block is kBN / R boxes of R = min(page_size, kBN) rows
-    uint64_t pd[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(Hkv),
-                      static_cast<uint64_t>(num_pages) * static_cast<uint64_t>(pages->page_size)};
-    uint64_t pstr[2] = {static_cast<uint64_t>(D) * kveb, static_cast<uint64_t>(Hkv) * D * kveb};
-    uint32_t pbox[3] = {64, 1, static_cast<uint32_t>(std::min(pages->page_size, bn))};
-    if ((rc = host::get_tmap(&tk, k, 3, pd, pstr, pbox, kvsw, kvdt))) return rc;
-    if ((rc = host::get_tmap(&tv, v, 3, pd, pstr, pbox, kvsw, kvdt))) return rc;
+    const uint64_t prows = static_cast<uint64_t>(num_pages) * static_cast<uint64_t>(pages->page_size);
+    const int R = std::min(pages->page_size, bn);
+    if ((rc = rows_map(&tk, k, D, Hkv, prows, R, kveb, kvdt, kvsw))) return rc;
+    if ((rc = rows_map(&tv, v, D, Hkv, prows, R, kveb, kvdt, kvsw))) return rc;
   } else {
     if ((rc = host::get_tmap(&tk, k, 3, kdims, kstr, kbox, kvsw, kvdt))) return rc;
     if (vt) {
@@ -473,6 +488,104 @@ int fmha_paged(const void* q, const void* k_cache, const void* v_cache, void* o,
                          static_cast<cudaStream_t>(stream), &lens, &pages, num_pages, v_scale);
 }
 
+// b200_fmha_fwd_{f16,bf16}_varlen (table == nullptr: cu_k is cu_seqlens_k, K / V [total_k, Hkv, D]) and _varlen_paged
+// (cu_k is seqused_k, K / V pools of num_pages pages [page_size, Hkv, D], total_k unused).  Every check comes before
+// the first CUDA call.  One launch of attn_varlen_kernel with the ring and shared memory of the seqlens kernels.
+template <typename T>
+int fmha_varlen(const char* who, const void* q, const void* k, const void* v, void* o, float* lse, const int* cu_q,
+                const int* cu_k, const int* table, int B, int H, int Hkv, int total_q, int total_k, int max_q, int max_k,
+                int num_pages, int page_size, int max_pages, int D, int causal, float scale, void* stream) {
+  const bool paged = table != nullptr;
+  if (!q || !k || !v || !o || !cu_q || !cu_k)
+    return fail(B200_EINVAL, paged ? "%s: null pointer (q, k_cache, v_cache, o, cu_seqlens_q, seqused_k and "
+                                     "block_table are required)"
+                                   : "%s: null pointer (q, k, v, o, cu_seqlens_q and cu_seqlens_k are required)",
+                who);
+  if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "%s: bad shape B=%d H=%d D=%d", who, B, H, D);
+  if (total_q <= 0) return fail(B200_EINVAL, "%s: total_q=%d must be >= 1", who, total_q);
+  if (!paged && total_k <= 0) return fail(B200_EINVAL, "%s: total_k=%d must be >= 1", who, total_k);
+  if (max_q <= 0) return fail(B200_EINVAL, "%s: max_seqlen_q=%d must be >= 1", who, max_q);
+  if (!paged && max_k <= 0) return fail(B200_EINVAL, "%s: max_seqlen_k=%d must be >= 1", who, max_k);
+  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "%s: causal must be 0 or 1, got %d", who, causal);
+  if (Hkv <= 0 || H % Hkv != 0) return fail(B200_EINVAL, "%s: Hkv=%d must be >= 1 and divide H=%d", who, Hkv, H);
+  if (static_cast<long long>(B) * Hkv > 65535)
+    return fail(B200_EINVAL, "%s: B*Hkv = %lld exceeds the grid limit 65535", who, static_cast<long long>(B) * Hkv);
+  if ((reinterpret_cast<uintptr_t>(cu_q) & 3u) != 0)
+    return fail(B200_EINVAL, "%s: cu_seqlens_q must be 4-byte aligned (int32)", who);
+  if ((reinterpret_cast<uintptr_t>(cu_k) & 3u) != 0)
+    return fail(B200_EINVAL, paged ? "%s: seqused_k must be 4-byte aligned (int32)"
+                                   : "%s: cu_seqlens_k must be 4-byte aligned (int32)", who);
+  if (paged) {
+    if ((reinterpret_cast<uintptr_t>(table) & 3u) != 0)
+      return fail(B200_EINVAL, "%s: block_table must be 4-byte aligned (int32)", who);
+    if (num_pages < 1) return fail(B200_EINVAL, "%s: num_pages=%d must be >= 1", who, num_pages);
+    if (max_pages < 1) return fail(B200_EINVAL, "%s: max_pages_per_seq=%d must be >= 1", who, max_pages);
+    if (page_size < 16 || (page_size & (page_size - 1)) != 0)
+      return fail(B200_EINVAL, "%s: page_size=%d must be a power of two >= 16", who, page_size);
+    if (static_cast<long long>(num_pages) * page_size > 0x7FFFFFFFll)
+      return fail(B200_EINVAL, "%s: num_pages*page_size = %lld pool rows exceed 2^31 - 1", who,
+                  static_cast<long long>(num_pages) * page_size);
+    if (static_cast<long long>(max_pages) * page_size > 0x7FFFFFFFll)
+      return fail(B200_EINVAL, "%s: max_pages_per_seq*page_size = %lld keys per sequence exceed 2^31 - 1", who,
+                  static_cast<long long>(max_pages) * page_size);
+  }
+  if (D % 8 != 0) return fail(B200_ENOTSUP, "%s: headdim not support! (D=%d must be a multiple of 8)", who, D);
+  if (D > 1024) return fail(B200_ENOTSUP, "%s: headdim not support! (D=%d > 1024)", who, D);
+  // the bytes of q / o must be addressable in int64 (k / v: rows < 2^31 times Hkv <= 65535 times D <= 1024 are)
+  if (static_cast<long long>(total_q) * H > 0x3FFFFFFFFFFFFFFFll / D)
+    return fail(B200_EINVAL, "%s: total_q*H*D = %d*%d*%d elements overflow", who, total_q, H, D);
+  const long long kv_rows = paged ? static_cast<long long>(num_pages) * page_size : total_k;
+  const int G = H / Hkv;
+  if (static_cast<long long>(G) * max_q > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "%s: (H/Hkv)*max_seqlen_q = %lld query rows per K/V head exceed 2^31 - 1", who,
+                static_cast<long long>(G) * max_q);
+  const Family f = family(D);
+  const int tph = (max_q + 64 * f.wgs - 1) / (64 * f.wgs), slabs = (D + f.ds - 1) / f.ds;
+  if (static_cast<long long>(G) * tph * slabs > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "%s: (H/Hkv)*ceil(max_seqlen_q/%d)*%d = %lld CTAs exceed the grid limit 2^31 - 1", who,
+                64 * f.wgs, slabs, static_cast<long long>(G) * tph * slabs);
+  if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
+
+  const int nk_pad = paged ? max_pages * page_size : max_k;   // the clamp of every sequence's keys
+  attn::Params p;
+  p.Nq = G * max_q;
+  p.qpos = max_q;
+  p.Nk = nk_pad;
+  p.D = D;
+  p.nq = (D + 63) / 64;
+  p.num_kv = (nk_pad + f.bn - 1) / f.bn;
+  p.diag = nk_pad - max_q;
+  p.slabs = slabs;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.lse = lse;
+  p.rms_g = 0.f;
+  p.o_ptr = static_cast<__half*>(o);
+  p.ws_o = nullptr;
+  p.ws_lse = nullptr;
+  p.tph = tph;
+  const int smem = ring_smem(f, p.nq, false, 0, &p.ring);
+  if (smem == 0) return fail(B200_ENOTSUP, "%s: headdim not support! (D=%d)", who, D);
+
+  constexpr bool bf16 = std::is_same_v<T, __nv_bfloat16>;
+  const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMap tq, tk, tv;
+  int rc;
+  if ((rc = rows_map(&tq, q, D, H, static_cast<uint64_t>(total_q), 64, 2, dt))) return rc;
+  const int box = paged ? std::min(page_size, f.bn) : f.bn;
+  if ((rc = rows_map(&tk, k, D, Hkv, static_cast<uint64_t>(kv_rows), box, 2, dt))) return rc;
+  if ((rc = rows_map(&tv, v, D, Hkv, static_cast<uint64_t>(kv_rows), box, 2, dt))) return rc;
+  const attn::Varlen vl{cu_q, cu_k, total_q, H, Hkv};
+  const attn::Pages pages{table, page_size, max_pages};
+  const attn::Pages* pg = paged ? &pages : nullptr;
+  const int bh = B * Hkv, qtiles = G * tph;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (f.ds == 64)
+    return attn::launch_attn_varlen<T, 64, 128, 2>(tq, tk, tv, p, qtiles, bh, smem, causal == 1, vl, pg, st);
+  if (f.ds == 128)
+    return attn::launch_attn_varlen<T, 128, 64, 2>(tq, tk, tv, p, qtiles, bh, smem, causal == 1, vl, pg, st);
+  return attn::launch_attn_varlen<T, 256, 64, 1>(tq, tk, tv, p, qtiles, bh, smem, causal == 1, vl, pg, st);
+}
+
 }  // namespace
 
 extern "C" {
@@ -590,6 +703,41 @@ int b200_fmha_fwd_bf16_fp8kv_paged(const void* q, const void* k_cache, const voi
   return fmha_paged<__nv_bfloat16, __nv_fp8_e4m3>(q, k_cache, v_cache, o, lse, block_table, seqlens_q, seqlens_k, B, H,
                                                   Hkv, Nq, num_pages, page_size, max_pages_per_seq, D, causal,
                                                   num_splits, scale, stream, k_scale, v_scale);
+}
+
+int b200_fmha_fwd_f16_varlen(const void* q, const void* k, const void* v, void* o, float* lse, const int* cu_seqlens_q,
+                             const int* cu_seqlens_k, int B, int H, int Hkv, int total_q, int total_k, int max_seqlen_q,
+                             int max_seqlen_k, int D, int causal, float scale, void* stream) {
+  return fmha_varlen<__half>("fmha_varlen", q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k, nullptr, B, H, Hkv, total_q,
+                             total_k, max_seqlen_q, max_seqlen_k, 0, 0, 0, D, causal, scale, stream);
+}
+
+int b200_fmha_fwd_bf16_varlen(const void* q, const void* k, const void* v, void* o, float* lse, const int* cu_seqlens_q,
+                              const int* cu_seqlens_k, int B, int H, int Hkv, int total_q, int total_k,
+                              int max_seqlen_q, int max_seqlen_k, int D, int causal, float scale, void* stream) {
+  return fmha_varlen<__nv_bfloat16>("fmha_varlen", q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k, nullptr, B, H, Hkv,
+                                    total_q, total_k, max_seqlen_q, max_seqlen_k, 0, 0, 0, D, causal, scale, stream);
+}
+
+// block_table is checked here: a null one would turn the call into the packed one
+int b200_fmha_fwd_f16_varlen_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
+                                   const int* cu_seqlens_q, const int* seqused_k, const int* block_table, int B, int H,
+                                   int Hkv, int total_q, int max_seqlen_q, int num_pages, int page_size,
+                                   int max_pages_per_seq, int D, int causal, float scale, void* stream) {
+  if (!block_table) return fail(B200_EINVAL, "fmha_varlen_paged: null pointer (block_table is required)");
+  return fmha_varlen<__half>("fmha_varlen_paged", q, k_cache, v_cache, o, lse, cu_seqlens_q, seqused_k, block_table, B,
+                             H, Hkv, total_q, 0, max_seqlen_q, 0, num_pages, page_size, max_pages_per_seq, D, causal,
+                             scale, stream);
+}
+
+int b200_fmha_fwd_bf16_varlen_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
+                                    const int* cu_seqlens_q, const int* seqused_k, const int* block_table, int B, int H,
+                                    int Hkv, int total_q, int max_seqlen_q, int num_pages, int page_size,
+                                    int max_pages_per_seq, int D, int causal, float scale, void* stream) {
+  if (!block_table) return fail(B200_EINVAL, "fmha_varlen_paged: null pointer (block_table is required)");
+  return fmha_varlen<__nv_bfloat16>("fmha_varlen_paged", q, k_cache, v_cache, o, lse, cu_seqlens_q, seqused_k,
+                                    block_table, B, H, Hkv, total_q, 0, max_seqlen_q, 0, num_pages, page_size,
+                                    max_pages_per_seq, D, causal, scale, stream);
 }
 
 int b200_fmha_fwd_f16_rmsnorm(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H,

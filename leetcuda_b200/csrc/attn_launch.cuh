@@ -1,5 +1,6 @@
 // attn_launch.cuh — the host launch of one attention kernel, shared by attn_capi.cu (the C entries and the fp16
-// kernels) and attn_bf16.cu (the bf16 kernels, a translation unit of their own so that the two compile in parallel).
+// kernels) and the translation units of the other kernels (attn_bf16.cu, attn_fp8kv_*.cu, attn_varlen.cu), which
+// compile in parallel.
 #pragma once
 #include <string.h>
 
@@ -51,6 +52,12 @@ template <typename T, int kDS, int kBN, int kWG>
 int launch_attn_fp8kv(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const Params& p, int qtiles,
                       int BH, int smem, bool causal, int splits, const Lens& lens, const Pages* pages, float v_scale,
                       cudaStream_t stream);
+
+// The packed variable-length kernel of the family (kDS, kBN, kWG) with T = __half or __nv_bfloat16 (attn_varlen.cu):
+// attn_varlen_kernel with paged K/V when pages is given, else with packed K/V.
+template <typename T, int kDS, int kBN, int kWG>
+int launch_attn_varlen(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const Params& p, int qtiles,
+                       int BH, int smem, bool causal, const Varlen& vl, const Pages* pages, cudaStream_t stream);
 
 }  // namespace attn
 }  // namespace b200

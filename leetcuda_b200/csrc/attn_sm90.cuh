@@ -58,6 +58,11 @@
 //     their keys are masked and their V rows zeroed, since the partial key block's V rows past Lk_b come from real pages
 //     (zeroed whenever Lk_b % kBN != 0, not only below the padded Nk);
 //   * a page id is only a TMA coordinate: one outside [0, num_pages) reads zeros (wrong values, no out-of-bounds access).
+//
+// Packed variable-length sequences (attn_varlen_kernel, b200_fmha_fwd_{f16,bf16}_varlen[_paged]): token-major Q, O
+// [total_q, H, D] and lse [H, total_q], sequence b at rows cu_q[b] ..; K/V [total_k, Hkv, D] at rows cu_k[b] .., or
+// paged.  The per-sequence-length kernel with per-head tiles and token-major addresses (the end of this file); a tile
+// past Lq_b exits before its first load, and only rows t < Lq_b inside [0, total_q) are stored.
 #pragma once
 #include <cuda.h>
 
@@ -102,6 +107,16 @@ struct Pages {
   int max_pages;
 };
 
+// attn_varlen_kernel: token-major Q / O [total_q, h, D] and lse [h, total_q]; sequence b is rows cu_q[b] .. cu_q[b+1]-1
+// of them, and (packed K/V) rows cu_k[b] .. cu_k[b+1]-1 of K and V [total_k, hkv, D].  Paged K/V: k_used[b] keys.
+struct Varlen {
+  const int* cu_q;     // int32 [B + 1]
+  const int* cu_k;     // packed K/V: int32 [B + 1]; paged K/V: seqused_k, int32 [B]
+  int total_q;         // rows of Q and O
+  int h;               // query heads
+  int hkv;             // K/V heads (grid.y = b * hkv + K/V head)
+};
+
 // Keys whose exponential the D <= 128 kernels evaluate on the FMA pipe (exp2_fma_pipe) instead of MUFU.EX2: bit i
 // selects the key pair (2i, 2i + 1) of every 32 keys.  A thread holds the pairs 8 jj + 2 (lane % 4), i.e. pair
 // 4 (jj % 4) + lane % 4, so a selection that is uniform over a warp takes whole nibbles.
@@ -119,6 +134,12 @@ struct Pages {
 
 template <int kWG>
 constexpr int threads() { return 128 * (kWG + 1); }
+
+// kVarlen: TMA row coordinate `first + t` of a sequence that starts at row `first` (device data): wraps instead of
+// overflowing, and TMA reads zeros for any row outside the tensor
+__device__ __forceinline__ int vrow(int first, int t) {
+  return static_cast<int>(static_cast<unsigned>(first) + static_cast<unsigned>(t));
+}
 
 // one ring slot: a {64 columns, bn keys} chunk of K or V, or a {64 keys, ds columns} chunk of V^T
 __host__ __device__ constexpr int slot_bytes(int bn, int ds, bool vt) { return 128 * (vt && ds > bn ? ds : bn); }
@@ -183,15 +204,19 @@ __device__ __forceinline__ int2 kv_blocks(const Params& p, int q0, int row_end, 
 // element type of Q, K, V and O, __half or __nv_bfloat16 (the top of this file; natural V only for bf16).
 // kFP8: K and V are e4m3 bytes, staged by TMA and widened to T in shared memory by producer warps 1-3 (the end of
 // this file); v_scale multiplies the normalised fp32 O before its rounding to T.
+// kVarlen: token-major Q, O and lse through `vl`, K/V packed by cu_k or paged (the end of this file); implies kSeqlens
+// and kGQA, per-head tiles (p.tph > 0) and no split.
 template <int kDS, int kBN, int kWG, bool kVT, bool kCausal, bool kGQA, bool kSplit, bool kSeqlens, bool kPaged = false,
-          typename T = __half, bool kFP8 = false>
+          typename T = __half, bool kFP8 = false, bool kVarlen = false>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k,
                                               const CUtensorMap& tmap_v, Params p, const Lens& lens,
-                                              const Pages& pages = Pages{}, float v_scale = 1.f) {
+                                              const Pages& pages = Pages{}, float v_scale = 1.f,
+                                              const Varlen& vl = Varlen{}) {
   static_assert(!kVT || kDS <= 128, "transposed V: one slab of <= 128 columns");
   static_assert(!kSeqlens || (!kVT && kGQA), "per-sequence lengths: natural V, query positions of packed rows");
   static_assert(!kPaged || kSeqlens, "paged K/V: per-sequence lengths");
   static_assert(!kFP8 || kSeqlens, "fp8 K/V: the per-sequence-length and paged kernels");
+  static_assert(!kVarlen || (kSeqlens && !kSplit && !kFP8), "varlen: per-sequence lengths, no split, fp16 / bf16 K/V");
   constexpr bool kBF16 = std::is_same_v<T, __nv_bfloat16>;
   static_assert(kBF16 || std::is_same_v<T, __half>, "elements: fp16 or bf16");
   static_assert(!kBF16 || !kVT, "bf16: natural V");
@@ -226,7 +251,16 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
   const int qtile = kCausal ? gridDim.x / p.slabs - 1 - blockIdx.x / p.slabs : blockIdx.x / p.slabs;
   int q0 = qtile * 64 * kWG;
   int row_end = p.Nq, off = 0;   // kGQA: the rows this CTA stores end before row_end; query position = row - off
-  if constexpr (kCausal && kGQA) {
+  [[maybe_unused]] int qh = 0, vhk = 0;   // kVarlen: the CTA's query head and K/V head
+  if constexpr (kVarlen) {
+    // per-head tiles with or without the mask; causal: the longest first across the G heads, as below
+    const int x = blockIdx.x / p.slabs, G = gridDim.x / p.slabs / p.tph;
+    off = (x % G) * p.qpos;
+    q0 = off + (kCausal ? p.tph - 1 - x / G : x / G) * 64 * kWG;
+    row_end = off + p.qpos;
+    vhk = blockIdx.y % vl.hkv;
+    qh = vhk * G + x % G;
+  } else if constexpr (kCausal && kGQA) {
     if (p.tph > 0) {
       // per-head tiles, the longest first across the G heads of the group, not only within one
       const int x = blockIdx.x / p.slabs, G = gridDim.x / p.slabs / p.tph;
@@ -241,7 +275,26 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
   // kSeqlens: this sequence's valid query positions lq and keys p.Nk (nk_pad: the padded Nk of the K/V buffers)
   int lq = 0;
   [[maybe_unused]] const int nk_pad = p.Nk;
-  if constexpr (kSeqlens) {
+  // kVarlen: the sequence's first row of Q / O and (packed K/V) of K / V
+  [[maybe_unused]] int qs = 0, ks = 0;
+  if constexpr (kVarlen) {
+    const int b = blockIdx.y / vl.hkv;
+    qs = __ldg(vl.cu_q + b);
+    lq = static_cast<int>(min(max(static_cast<long long>(__ldg(vl.cu_q + b + 1)) - qs, 0ll),
+                              static_cast<long long>(p.qpos)));
+    long long lk;
+    if constexpr (kPaged) {
+      lk = __ldg(vl.cu_k + b);
+    } else {
+      ks = __ldg(vl.cu_k + b);
+      lk = static_cast<long long>(__ldg(vl.cu_k + b + 1)) - ks;
+    }
+    p.Nk = static_cast<int>(min(max(lk, 0ll), static_cast<long long>(nk_pad)));
+    p.diag = p.Nk - lq;
+    p.num_kv = (p.Nk + kBN - 1) / kBN;
+    // a tile of positions past the sequence: nothing to load, nothing to store (uniform over the CTA, no cluster)
+    if (q0 - off >= lq) return;
+  } else if constexpr (kSeqlens) {
     const int b = blockIdx.y / lens.hkv;
     lq = lens.q ? min(max(__ldg(lens.q + b), 0), p.qpos) : p.qpos;
     const int lk = lens.k ? min(max(__ldg(lens.k + b), 0), nk_pad) : nk_pad;
@@ -259,7 +312,8 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
   [[maybe_unused]] const uint32_t vbar = rowss;   // its V chunks land here (no fused RMS norm with kSeqlens)
   // kFP8: the converters write those rows as zeros instead (vz stays -1)
   if constexpr (kSeqlens && !kFP8) {
-    if (p.Nk % kBN != 0 && (kPaged || p.Nk < nk_pad) && p.num_kv - 1 >= kv.x && p.num_kv - 1 < kv.y) vz = p.num_kv - 1;
+    if (p.Nk % kBN != 0 && (kPaged || kVarlen || p.Nk < nk_pad) && p.num_kv - 1 >= kv.x && p.num_kv - 1 < kv.y)
+      vz = p.num_kv - 1;
   }
 
   if (threadIdx.x == 0) {
@@ -295,8 +349,13 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
           prefetch_tmap(&tmap_v);
           mbar_expect_tx(qbar, kWG * p.nq * 8192);
           for (int w = 0; w < kWG; ++w)
-            for (int c = 0; c < p.nq; ++c)
-              tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, q0 + 64 * w, bh, kEvictFirst);
+            for (int c = 0; c < p.nq; ++c) {
+              if constexpr (kVarlen)
+                tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, qh, vrow(qs, q0 - off + 64 * w),
+                            kEvictFirst);
+              else
+                tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, q0 + 64 * w, bh, kEvictFirst);
+            }
         }
         int it = 0;
         int row = kv.x < kv.y ? pool_row(kv.x) : 0;
@@ -330,8 +389,13 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
       prefetch_tmap(&tmap_v);
       mbar_expect_tx(qbar, kWG * p.nq * 8192);
       for (int w = 0; w < kWG; ++w)
-        for (int c = 0; c < p.nq; ++c)
-          tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, q0 + 64 * w, bh, kEvictFirst);
+        for (int c = 0; c < p.nq; ++c) {
+          if constexpr (kVarlen)
+            tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, qh, vrow(qs, q0 - off + 64 * w),
+                        kEvictFirst);
+          else
+            tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, q0 + 64 * w, bh, kEvictFirst);
+        }
       int it = 0;
       // kFP8: every K / V chunk goes to the staging slot s, onto staged(s)
       auto landed = [&](int s) { return kFP8 ? staged(s) : full(s); };
@@ -346,7 +410,10 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
       for (int j = kv.x; j < kv.y; ++j) {
         for (int c = 0; c < p.nq; ++c) {
           const int s = next(KV_BYTES);
-          tma_load_3d(dst(s), &tmap_k, landed(s), 64 * c, j * kBN, bh, kEvictLast);
+          if constexpr (kVarlen)
+            tma_load_3d(dst(s), &tmap_k, landed(s), 64 * c, vhk, vrow(ks, j * kBN), kEvictLast);
+          else
+            tma_load_3d(dst(s), &tmap_k, landed(s), 64 * c, j * kBN, bh, kEvictLast);
         }
         for (int c = 0; c < nvc; ++c) {
           if constexpr (kVT) {
@@ -360,12 +427,18 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
                 if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
                 ++it;
                 if (c == 0) mbar_expect_tx(vbar, nvc * KV_BYTES);
-                tma_load_3d(sring + s * SLOT, &tmap_v, vbar, d0 + 64 * c, j * kBN, bh, kEvictLast);
+                if constexpr (kVarlen)
+                  tma_load_3d(sring + s * SLOT, &tmap_v, vbar, d0 + 64 * c, vhk, vrow(ks, j * kBN), kEvictLast);
+                else
+                  tma_load_3d(sring + s * SLOT, &tmap_v, vbar, d0 + 64 * c, j * kBN, bh, kEvictLast);
                 continue;
               }
             }
             const int s = next(KV_BYTES);
-            tma_load_3d(dst(s), &tmap_v, landed(s), d0 + 64 * c, j * kBN, bh, kEvictLast);
+            if constexpr (kVarlen)
+              tma_load_3d(dst(s), &tmap_v, landed(s), d0 + 64 * c, vhk, vrow(ks, j * kBN), kEvictLast);
+            else
+              tma_load_3d(dst(s), &tmap_v, landed(s), d0 + 64 * c, j * kBN, bh, kEvictLast);
           }
         }
       }
@@ -665,6 +738,32 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
       return;
     }
   }
+  if constexpr (kVarlen) {
+    // token-major O row cu_q[b] + t of head qh and lse [h, total_q]: only positions t < Lq_b of rows inside
+    // [0, total_q) are stored (the rows past them belong to the next sequence or to none); a row without a visible key
+    // gets literal 0 and -inf
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int t = q0 + 64 * w + 16 * warp + lane / 4 + 8 * i - off;
+      const long long grow = static_cast<long long>(qs) + t;
+      if (t >= lq || grow < 0 || grow >= vl.total_q) continue;
+      const bool none = m[i] == -INFINITY;
+      if (p.lse && slab == 0 && (lane % 4) == 0)
+        p.lse[static_cast<size_t>(qh) * vl.total_q + grow] =
+            none ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
+      T* orow = reinterpret_cast<T*>(p.o_ptr) + (static_cast<size_t>(grow) * vl.h + qh) * p.D;
+#pragma unroll
+      for (int c = 0; c < NDC; ++c)
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
+          if (col < p.D)
+            *reinterpret_cast<uint32_t*>(orow + col) =
+                none ? 0u : pack(o[c][4 * jj + 2 * i] * inv[i], o[c][4 * jj + 2 * i + 1] * inv[i]);
+        }
+    }
+    return;
+  }
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     if (p.rms_g > 0.f) inv[i] *= rsqrtf(ss[i] / static_cast<float>(p.D) + 1e-5f) * p.rms_g;
@@ -770,6 +869,26 @@ attn_fwd_fp8kv_paged_kernel(const __grid_constant__ CUtensorMap tmap_q, const __
                             const Pages pages, const float v_scale) {
   attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, kSplit, true, true, T, true>(tmap_q, tmap_k, tmap_v, p, lens,
                                                                                  pages, v_scale);
+}
+
+// Packed variable-length sequences (b200_fmha_fwd_{f16,bf16}_varlen, _varlen_paged): token-major Q and O
+// [total_q, H, D], lse [H, total_q], sequence b at rows cu_q[b] ..; K/V [total_k, Hkv, D] at rows cu_k[b] .. (kPagedKV
+// false) or paged pools read through the paged producer (kPagedKV true, lengths seqused_k).  The per-sequence-length
+// kernel in every other respect, with p.qpos = max_seqlen_q and p.Nk = max_seqlen_k (paged: max_pages * page_size).
+//   * grid (G * tph * slabs, B * Hkv): per-head tiles whatever the mask (tph = ceil(max_seqlen_q / (64 kWG))), causal
+//     the longest first; a tile whose first position is >= Lq_b returns before it initialises a barrier;
+//   * Q: a {D, H, total_q} tensor map, box {64, 1, 64}: chunk c of warpgroup w at (64 c, head, cu_q[b] + t0 + 64 w);
+//     packed K/V: {D, Hkv, total_k}, box {64, 1, kBN}: key block j at row cu_k[b] + j kBN (rows of the next sequence
+//     in the partial block are masked in S and zeroed in V, as under kPaged);
+//   * the epilogue stores only positions t < Lq_b of rows cu_q[b] + t inside [0, total_q), indexed in size_t.
+// T in the template arguments carries the element type (the kernel's name has no "bf16" in it).  Instantiated in
+// attn_varlen.cu.
+template <int kDS, int kBN, int kWG, bool kCausal, bool kPagedKV, typename T>
+__global__ void __launch_bounds__(threads<kWG>(), 1)
+attn_varlen_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                   const __grid_constant__ CUtensorMap tmap_v, const Params p, const Varlen vl, const Pages pages) {
+  attn_fwd_body<kDS, kBN, kWG, false, kCausal, true, false, true, kPagedKV, T, false, true>(
+      tmap_q, tmap_k, tmap_v, p, Lens{nullptr, nullptr, vl.hkv}, pages, 1.f, vl);
 }
 
 }  // namespace attn

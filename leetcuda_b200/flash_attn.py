@@ -296,6 +296,118 @@ def _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlen
     _call_on_device(getattr(_capi.lib(), name + "_paged"), args, Q.device.index)
 
 
+def fmha_varlen_fwd(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q: int, max_seqlen_k: int, *,
+                    scale: float = 0.0, causal: bool = False, lse=None, block_table=None, seqused_k=None,
+                    num_splits: int = 1, v_transposed: bool = False, rms_g: float = 0.0) -> None:
+    """Packed variable-length attention, FlashAttention's ``flash_attn_varlen_func`` layout, on the current CUDA stream
+    of ``q``'s device (``b200_fmha_fwd_{f16,bf16}_varlen``; with ``block_table``: ``..._varlen_paged``).
+
+    ``q``, ``o`` are ``[total_q, H, D]`` and ``k``, ``v`` ``[total_k, Hkv, D]``, fp16 or bf16 (one dtype for all four),
+    contiguous, with Hkv dividing H (query head h reads K/V head ``h // (H // Hkv)``).  ``cu_seqlens_q`` and
+    ``cu_seqlens_k`` are int32 contiguous CUDA tensors ``[B + 1]``: sequence b has
+    ``Lq_b = clamp(cu_seqlens_q[b+1] - cu_seqlens_q[b], 0, max_seqlen_q)`` queries at rows ``cu_seqlens_q[b] + t`` and
+    ``Lk_b = clamp(cu_seqlens_k[b+1] - cu_seqlens_k[b], 0, max_seqlen_k)`` keys at rows ``cu_seqlens_k[b] + t``.
+    ``causal=True`` masks key j for query i when ``j > i + (Lk_b - Lq_b)`` (bottom-right, per sequence, as
+    ``fmha_fwd(seqlens_q=, seqlens_k=)``).  ``lse`` (optional) is fp32 ``[H, total_q]``, the layout of
+    ``merge_attn_states``, so the O and lse of two calls over disjoint keys merge without a reshape.
+
+    ``block_table`` (int32 ``[B, max_pages_per_seq]``) makes ``k`` and ``v`` paged pools
+    ``[num_pages, page_size, Hkv, D]`` as in ``fmha_fwd(block_table=)``: then ``cu_seqlens_k`` must be None,
+    ``seqused_k`` (int32 ``[B]``) gives ``Lk_b = clamp(seqused_k[b], 0, max_pages_per_seq * page_size)``,
+    ``max_seqlen_k`` is ignored, and key t of sequence b is row ``t % page_size`` of page ``block_table[b][t // page_size]``.
+
+    Only rows ``cu_seqlens_q[b] + t`` with ``t < Lq_b`` inside ``o`` are written: rows of ``o`` and columns of ``lse``
+    that belong to no sequence keep their contents.  Rows without a visible key get O = 0 and lse = -inf.  Keys of the
+    next sequence contribute nothing whatever they hold.  Offsets, lengths and tables are read on the GPU only (no host
+    synchronisation), so a captured CUDA graph replays with new values written into the same tensors.  The results are
+    bit for bit ``fmha_fwd(seqlens_q=, seqlens_k=, num_splits=1)`` (or the ``block_table`` call) on padded copies.
+
+    Every query head gets ``ceil(max_seqlen_q / 128)`` query tiles of its own (64-row tiles for D > 128).  A batch of
+    one-token decode rows therefore fills one row of every tile: use ``fmha_fwd`` with ``seqlens_q`` / ``block_table``
+    for decoding.  Not supported, and rejected by name: ``num_splits`` other than 1, fp8 K/V, ``v_transposed`` and the
+    fused RMS norm (``rms_g``)."""
+    if isinstance(num_splits, bool) or num_splits != 1:
+        raise RuntimeError(f"leetcuda_b200.flash_attn.fmha_varlen_fwd: num_splits={num_splits!r} is not supported "
+                           f"(varlen runs unsplit: num_splits must be 1)")
+    if v_transposed:
+        raise RuntimeError("leetcuda_b200.flash_attn.fmha_varlen_fwd: v_transposed=True is not supported (natural V "
+                           "[total_k, Hkv, D] only)")
+    if rms_g:
+        raise RuntimeError(f"leetcuda_b200.flash_attn.fmha_varlen_fwd: the fused RMS norm (rms_g={rms_g!r}) is not "
+                           f"supported with varlen")
+    who = "leetcuda_b200.flash_attn.fmha_varlen_fwd"
+    for name, t in (("q", q), ("k", k), ("v", v), ("o", o)):
+        if not isinstance(t, torch.Tensor):
+            raise RuntimeError(f"{who}: {name} must be a torch.Tensor")
+    if any(t.dtype in _FP8_DTYPES for t in (q, k, v, o)):
+        raise RuntimeError(f"{who}: fp8 K/V is not supported with varlen (use fmha_fwd with float8_e4m3fn K/V)")
+    dts = {t.dtype for t in (q, k, v, o)}
+    if len(dts) != 1 or q.dtype not in (torch.float16, torch.bfloat16):
+        raise RuntimeError(f"{who}: q, k, v and o must share one dtype, fp16 or bf16, got "
+                           + ", ".join(str(t.dtype).replace("torch.", "") for t in (q, k, v, o)))
+    if q.dim() != 3 or tuple(o.shape) != tuple(q.shape):
+        raise RuntimeError(f"{who}: q and o must be [total_q, H, D] of one shape, got q {tuple(q.shape)}, "
+                           f"o {tuple(o.shape)}")
+    total_q, H, D = q.shape
+    paged = block_table is not None
+    for name, x in (("max_seqlen_q", max_seqlen_q), ("max_seqlen_k", max_seqlen_k)):
+        if isinstance(x, bool) or not isinstance(x, int):
+            raise RuntimeError(f"{who}: {name} must be an int, got {x!r}")
+    if paged:
+        if cu_seqlens_k is not None:
+            raise RuntimeError(f"{who}: with block_table, cu_seqlens_k must be None (seqused_k gives the keys)")
+        if k.dim() != 4 or tuple(k.shape) != tuple(v.shape) or k.shape[3] != D or k.shape[2] < 1 or H % k.shape[2] \
+                or k.shape[0] < 1:
+            raise RuntimeError(f"{who}: with block_table, k and v must be pools [num_pages, page_size, Hkv, D] of the "
+                               f"same shape, with D = {D} and Hkv dividing H = {H}")
+        num_pages, page_size, Hkv, _ = k.shape
+        if page_size < 16 or page_size & (page_size - 1):
+            raise RuntimeError(f"{who}: page_size (k.shape[1]) must be a power of two >= 16, got {page_size}")
+    else:
+        if seqused_k is not None:
+            raise RuntimeError(f"{who}: seqused_k needs block_table (packed K/V take their lengths from cu_seqlens_k)")
+        if k.dim() != 3 or tuple(k.shape) != tuple(v.shape) or k.shape[2] != D or k.shape[1] < 1 or H % k.shape[1]:
+            raise RuntimeError(f"{who}: k and v must be [total_k, Hkv, D] of one shape, with D = {D} and Hkv dividing "
+                               f"H = {H}, got k {tuple(k.shape)}, v {tuple(v.shape)}")
+        total_k, Hkv, _ = k.shape
+    if lse is not None and (not isinstance(lse, torch.Tensor) or lse.dtype != torch.float32
+                            or tuple(lse.shape) != (H, total_q)):
+        raise RuntimeError(f"{who}: lse must be a contiguous fp32 CUDA tensor [H, total_q] = [{H}, {total_q}]")
+    if not isinstance(cu_seqlens_q, torch.Tensor) or cu_seqlens_q.dim() != 1 or cu_seqlens_q.shape[0] < 2:
+        raise RuntimeError(f"{who}: cu_seqlens_q must be an int32 contiguous CUDA tensor [B + 1] (B >= 1) on q's device")
+    B = cu_seqlens_q.shape[0] - 1
+    if paged:
+        t = block_table
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or t.dim() != 2 or t.shape[0] != B \
+                or t.shape[1] < 1 or not t.is_cuda or not t.is_contiguous() or t.device != q.device:
+            raise RuntimeError(f"{who}: block_table must be an int32 contiguous CUDA tensor "
+                               f"[B, max_pages_per_seq] = [{B}, >= 1] on q's device")
+    arrays = [("cu_seqlens_q", cu_seqlens_q, B + 1)]
+    arrays += [("seqused_k", seqused_k, B)] if paged else [("cu_seqlens_k", cu_seqlens_k, B + 1)]
+    for on_device in (False, True):   # every array's type and shape first, then where it lives
+        for name, t, n in arrays:
+            if not (isinstance(t, torch.Tensor) and t.dtype == torch.int32 and tuple(t.shape) == (n,)
+                    and t.is_contiguous()) or on_device and not (t.is_cuda and t.device == q.device):
+                raise RuntimeError(f"{who}: {name} must be an int32 contiguous CUDA tensor [{n}] on q's device")
+    for name, t in (("q", q), ("k", k), ("v", v), ("o", o)) + ((("lse", lse),) if lse is not None else ()):
+        if not t.is_cuda or t.device != q.device:
+            raise RuntimeError(f"{who}: {name} must be a CUDA tensor on q's device (no CPU path)")
+        if not t.is_contiguous():
+            raise RuntimeError(f"{who}: {name} must be contiguous")
+    name = "b200_fmha_fwd_bf16_varlen" if q.dtype == torch.bfloat16 else "b200_fmha_fwd_f16_varlen"
+    lse_ptr = None if lse is None else lse.data_ptr()
+    if paged:
+        args = [q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse_ptr, cu_seqlens_q.data_ptr(),
+                seqused_k.data_ptr(), block_table.data_ptr(), B, H, Hkv, total_q, int(max_seqlen_q), num_pages,
+                page_size, block_table.shape[1], D, int(bool(causal)), float(scale)]
+        name += "_paged"
+    else:
+        args = [q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse_ptr, cu_seqlens_q.data_ptr(),
+                cu_seqlens_k.data_ptr(), B, H, Hkv, total_q, total_k, int(max_seqlen_q), int(max_seqlen_k), D,
+                int(bool(causal)), float(scale)]
+    _call_on_device(getattr(_capi.lib(), name), args, q.device.index)
+
+
 def _call_on_device(fn, args, idx) -> None:
     if torch.cuda.current_device() != idx:
         with torch.cuda.device(idx):
@@ -382,4 +494,4 @@ def flash_attn_cute(Q, K, V, O) -> None:
     _fmha_one_length(Q, K, V, O)
 
 
-__all__ = OP_NAMES + ["flash_attn_cute", "fmha_fwd", "fmha_host", "OP_NAMES", "V_TRANSPOSED_OPS"]
+__all__ = OP_NAMES + ["flash_attn_cute", "fmha_fwd", "fmha_varlen_fwd", "fmha_host", "OP_NAMES", "V_TRANSPOSED_OPS"]

@@ -102,42 +102,48 @@ __global__ void __launch_bounds__(256) tf32_split3_kernel(const float* __restric
 // b[K,N] (fp32) -> bt[N, ld]: the TF32 wgmma reads both operands K-major, so the [K,N] layout of the reference's
 // SGEMM is restored to [N,K] first (HBM-bound, one pass).  mode 0: copy (ld = K); 1: also round b to TF32 in place
 // and copy the rounded value (ld = K); 2: the 3xTF32 split of b, bt[n, k] = hi, bt[n, K + k] = lo, bt[n, 2K + k] = hi
-// (ld = 3K; b is not written).
+// (ld = 3K; b is not written).  grid.y is capped at 65535 (K > 2,097,120 has more k-tiles than that): block y
+// transposes k-tiles blockIdx.y, blockIdx.y + gridDim.y, ...
 __global__ void __launch_bounds__(256) tf32_transpose_kernel(float* __restrict__ b, float* __restrict__ bt, int K, int N,
                                                              int mode) {
   __shared__ float tile[32][33];
-  const int n0 = blockIdx.x * 32, k0 = blockIdx.y * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int k = k0 + i, n = n0 + threadIdx.x;
-    if (k < K && n < N) {
-      float v = b[static_cast<size_t>(k) * N + n];
-      if (mode == 1) {
-        v = rna(v);
-        b[static_cast<size_t>(k) * N + n] = v;
-      }
-      tile[i][threadIdx.x] = v;
-    }
-  }
-  __syncthreads();
+  const int n0 = blockIdx.x * 32, k_tiles = (K + 31) / 32;
   const size_t ld = mode == 2 ? 3 * static_cast<size_t>(K) : K;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int n = n0 + i, k = k0 + threadIdx.x;
-    if (k >= K || n >= N) continue;
-    const float v = tile[threadIdx.x][i];
-    float* o = bt + static_cast<size_t>(n) * ld + k;
-    if (mode == 2) {
-      const float hi = rna(v), lo = rna(v - hi);
-      o[0] = hi;
-      o[K] = lo;
-      o[2 * static_cast<size_t>(K)] = hi;
-    } else {
-      o[0] = v;
+  for (int kt = blockIdx.y; kt < k_tiles; kt += gridDim.y) {
+    const int k0 = kt * 32;
+    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+      const int k = k0 + i, n = n0 + threadIdx.x;
+      if (k < K && n < N) {
+        float v = b[static_cast<size_t>(k) * N + n];
+        if (mode == 1) {
+          v = rna(v);
+          b[static_cast<size_t>(k) * N + n] = v;
+        }
+        tile[i][threadIdx.x] = v;
+      }
     }
+    __syncthreads();
+    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+      const int n = n0 + i, k = k0 + threadIdx.x;
+      if (k >= K || n >= N) continue;
+      const float v = tile[threadIdx.x][i];
+      float* o = bt + static_cast<size_t>(n) * ld + k;
+      if (mode == 2) {
+        const float hi = rna(v), lo = rna(v - hi);
+        o[0] = hi;
+        o[K] = lo;
+        o[2 * static_cast<size_t>(K)] = hi;
+      } else {
+        o[0] = v;
+      }
+    }
+    __syncthreads();   // the tile is refilled for the next k-tile
   }
 }
 
 int launch_tf32_transpose(const float* b, float* bt, int K, int N, int mode, cudaStream_t stream) {
-  dim3 grid((N + 31) / 32, (K + 31) / 32, 1), block(32, 8, 1);
+  const int k_tiles = (K + 31) / 32;
+  dim3 grid((N + 31) / 32, k_tiles < 65535 ? k_tiles : 65535, 1), block(32, 8, 1);
   tf32_transpose_kernel<<<grid, block, 0, stream>>>(const_cast<float*>(b), bt, K, N, mode);
   B200_CUDA_OK(cudaGetLastError());
   host::count_launch();
@@ -349,14 +355,19 @@ int b200_sgemm_tf32(float* a, float* b, float* c, int M, int N, int K, int b_lay
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool round = round_inputs_in_place != 0;
   int rc;
-  if (round && (rc = b200_tf32_round_inplace(a, static_cast<size_t>(M) * K, stream))) return rc;
   if (b_layout == B200_B_ROW_MAJOR_NK) {
+    if (round && (rc = b200_tf32_round_inplace(a, static_cast<size_t>(M) * K, stream))) return rc;
     if (round && (rc = b200_tf32_round_inplace(b, static_cast<size_t>(K) * N, stream))) return rc;
     return hgemm_impl(a, b, c, M, N, K, B200_B_ROW_MAJOR_NK, stream, nullptr, false, true);
   }
-  // [K,N]: round b in place (if asked) and transpose it into stream-ordered scratch in one pass
+  // [K,N]: round b in place (if asked) and transpose it into stream-ordered scratch in one pass.  The scratch is
+  // allocated first, so a call that cannot get it returns with a and b unchanged.
   float* bt = nullptr;
   B200_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&bt), static_cast<size_t>(K) * N * sizeof(float), stream));
+  if (round && (rc = b200_tf32_round_inplace(a, static_cast<size_t>(M) * K, stream))) {
+    cudaFreeAsync(bt, stream);
+    return rc;
+  }
   rc = launch_tf32_transpose(b, bt, K, N, round ? 1 : 0, stream);
   if (!rc) rc = hgemm_impl(a, bt, c, M, N, K, B200_B_ROW_MAJOR_NK, stream, nullptr, false, true);
   cudaFreeAsync(bt, stream);

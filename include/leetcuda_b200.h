@@ -310,6 +310,67 @@ int b200_fmha_fwd_bf16_varlen_paged(const void* q, const void* k_cache, const vo
                                     int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
                                     float scale, void* stream);
 
+/* ------------------------------------------------------------------ KV-cache append
+ * The write half of a decode or chunked-prefill step, in one launch (FlashAttention's flash_attn_with_kvcache append,
+ * vLLM's reshape_and_cache_flash): rotate q and the new k at each sequence's own positions, quantise k and v when the
+ * cache is e4m3, and scatter the new tokens into a dense or paged cache.  The attention call that follows takes
+ * seqlens_k = seqlens_out (b200_fmha_fwd_*_seqlens / _paged / _fp8kv_*).
+ *
+ * k_new, v_new: [B, Hkv, n_new, D] of T (f16 entries: fp16, bf16 entries: bf16).  cache_seqlens: int32 [B] in device
+ * memory.  Sequence b holds L_b = clamp(cache_seqlens[b], 0, capacity) tokens; new token t goes to position
+ * p = L_b + t, where capacity = Nk (dense) or max_pages_per_seq * page_size (paged).
+ *   dense: k_cache, v_cache [B, Hkv, Nk, D] (the layout of b200_fmha_fwd_f16_seqlens); row p of (b, h).
+ *   paged: pools [num_pages, page_size, Hkv, D] and block_table int32 [B, max_pages_per_seq] (the layout of
+ *          b200_fmha_fwd_f16_paged); row p % page_size of page block_table[b][p / page_size].  A table entry outside
+ *          [0, num_pages) means the token is not written.
+ * Tokens with p >= capacity are dropped; nothing is ever written out of bounds.  Every other cache byte keeps its value.
+ * cache_dtype: T's B200_DTYPE_F16 / B200_DTYPE_BF16 (the cache is T), or B200_DTYPE_E4M3: the cache holds
+ * cvt.rn.satfinite.e4m3(float(x) / scale) of the T value x (after rotary), an IEEE division, k_scale for k and v_scale
+ * for v — bit for bit torch's (x.float() / scale).clamp(-448, 448).to(torch.float8_e4m3fn).  The scales are per tensor,
+ * finite and > 0, and exactly 1 unless the cache is e4m3.
+ * seqlens_out (may be NULL): int32 [B], receives min(L_b + n_new, capacity), the key lengths of the attention call.
+ * q, q_out (both NULL or both set): [B, H, n_new, D] of T; q_out receives q rotated at the same positions p (every
+ * token, dropped or not); q_out == q rotates in place.  Without rotary tables q is copied.
+ * rotary_cos, rotary_sin (both NULL or both set): fp32 [rotary_len, rotary_dim / 2], indexed [p, i].  Pair i is
+ * (2i, 2i+1) with rotary_interleaved = 1 (GPT-J) and (i, i + rotary_dim / 2) with 0 (NeoX / Llama);
+ * x0' = x0 c - x1 s, x1' = x0 s + x1 c in fp32, rounded once to T; columns >= rotary_dim are copied; v is never rotated.
+ * Without tables rotary_dim, rotary_len and rotary_interleaved must be 0.
+ * Lengths and tables are read by the kernel only (no host copy, no synchronisation): a captured CUDA graph replays with
+ * the lengths the arrays hold at replay time.  Two sequences that write the same row of a shared page race; the
+ * library does not detect it.
+ * Checks (B200_EINVAL, message naming the argument, before any CUDA call): pointers; B, H, Hkv, n_new, D, Nk
+ * (num_pages, page_size, max_pages_per_seq) >= 1; H % Hkv == 0; cache_dtype; D % 8 == 0 (D % 16 == 0 for e4m3);
+ * page_size a power of two >= 16; capacity + n_new <= 2^31 - 1 and B * n_new * (2 Hkv + H) <= 2^31 - 1;
+ * rotary_dim % 16 == 0 and 0 < rotary_dim <= D; rotary_len >= capacity + n_new (positions come from device memory);
+ * the scales; tensors 16-byte aligned, int arrays 4-byte aligned; every buffer the call writes (k_cache, v_cache,
+ * q_out unless it is q, seqlens_out) disjoint from every other buffer.  One launch. */
+int b200_kvcache_append_f16(const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                            const int* cache_seqlens, int* seqlens_out /* may be NULL */, const void* q /* may be NULL */,
+                            void* q_out /* may be NULL */, const float* rotary_cos /* may be NULL */,
+                            const float* rotary_sin /* may be NULL */, int B, int H, int Hkv, int n_new, int Nk, int D,
+                            int rotary_dim, int rotary_len, int rotary_interleaved, int cache_dtype, float k_scale,
+                            float v_scale, void* stream);
+int b200_kvcache_append_bf16(const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                             const int* cache_seqlens, int* seqlens_out /* may be NULL */, const void* q /* may be NULL */,
+                             void* q_out /* may be NULL */, const float* rotary_cos /* may be NULL */,
+                             const float* rotary_sin /* may be NULL */, int B, int H, int Hkv, int n_new, int Nk, int D,
+                             int rotary_dim, int rotary_len, int rotary_interleaved, int cache_dtype, float k_scale,
+                             float v_scale, void* stream);
+int b200_kvcache_append_f16_paged(const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                                  const int* block_table, const int* cache_seqlens, int* seqlens_out /* may be NULL */,
+                                  const void* q /* may be NULL */, void* q_out /* may be NULL */,
+                                  const float* rotary_cos /* may be NULL */, const float* rotary_sin /* may be NULL */,
+                                  int B, int H, int Hkv, int n_new, int num_pages, int page_size, int max_pages_per_seq,
+                                  int D, int rotary_dim, int rotary_len, int rotary_interleaved, int cache_dtype,
+                                  float k_scale, float v_scale, void* stream);
+int b200_kvcache_append_bf16_paged(const void* k_new, const void* v_new, void* k_cache, void* v_cache,
+                                   const int* block_table, const int* cache_seqlens, int* seqlens_out /* may be NULL */,
+                                   const void* q /* may be NULL */, void* q_out /* may be NULL */,
+                                   const float* rotary_cos /* may be NULL */, const float* rotary_sin /* may be NULL */,
+                                   int B, int H, int Hkv, int n_new, int num_pages, int page_size,
+                                   int max_pages_per_seq, int D, int rotary_dim, int rotary_len, int rotary_interleaved,
+                                   int cache_dtype, float k_scale, float v_scale, void* stream);
+
 /* ------------------------------------------------------------------ SGEMM (TF32)
  * C[M,N] (fp32) = A[M,K] (fp32) x B on the tensor cores through wgmma .tf32 with fp32
  * accumulation — the sibling of the HGEMM path (SURVEY §8f-2).  Replaces
@@ -353,6 +414,7 @@ int b200_tf32_round_inplace(float* x, size_t n, void* stream);
 #define B200_DTYPE_F32 0
 #define B200_DTYPE_F16 1
 #define B200_DTYPE_BF16 2
+#define B200_DTYPE_E4M3 3 /* OCP e4m3 (torch.float8_e4m3fn): KV caches of b200_kvcache_append_* only */
 int b200_merge_attn_states(void* output, float* output_lse, const void* prefix_output,
                            const float* prefix_lse, const void* suffix_output, const float* suffix_lse,
                            int num_tokens, int num_heads, int head_size, int dtype, void* stream);

@@ -20,6 +20,7 @@ B200_OK = 0
 B_ROW_MAJOR_KN = 0  # "NN"
 B_ROW_MAJOR_NK = 1  # "TN"
 FMHA_MAX_SPLITS = 64  # B200_FMHA_MAX_SPLITS
+DTYPE_F16, DTYPE_BF16, DTYPE_E4M3 = 1, 2, 3  # B200_DTYPE_*
 
 _lib = None
 
@@ -61,6 +62,14 @@ SIGNATURES = {
                                             _i, _f, _vp]),
     "b200_fmha_fwd_bf16_varlen_paged": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i,
                                              _i, _f, _vp]),
+    "b200_kvcache_append_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i,
+                                     _i, _f, _f, _vp]),
+    "b200_kvcache_append_bf16": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i,
+                                      _i, _i, _f, _f, _vp]),
+    "b200_kvcache_append_f16_paged": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i,
+                                           _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
+    "b200_kvcache_append_bf16_paged": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i,
+                                            _i, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
     "b200_fmha_fwd_f16_rmsnorm":(_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
     "b200_rope_f32": (_i, [_vp, _vp, _i, _i, _vp]),
     "b200_rope_qk_f16": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),

@@ -357,6 +357,15 @@ B200_DEVICE uint2 e4m3x4_to_half2x2(uint32_t x) {
       : "r"(x));
   return r;
 }
+// two fp32 values to e4m3 codes, round to nearest even, saturated to +-448 (NaN stays NaN): lo in byte 0, hi in byte 1
+// (F2FP.SATFINITE.E4M3.F32.PACK_AB_MERGE_C on sm_90a)
+B200_DEVICE uint32_t float2_to_e4m3x2(float lo, float hi) {
+  uint32_t r;
+  asm("{\n\t.reg .b16 c;\n\tcvt.rn.satfinite.e4m3x2.f32 c, %1, %2;\n\tcvt.u32.u16 %0, c;\n\t}"
+      : "=r"(r)
+      : "f"(hi), "f"(lo));
+  return r;
+}
 // the same as bf16x2: through fp16 and fp32, both exact (an e4m3 value has 4 significant bits and an exponent inside
 // bf16's range), so every value, NaN included, keeps its value
 B200_DEVICE uint32_t half2_to_bf162(uint32_t h) {

@@ -19,6 +19,8 @@ always accumulate in fp32 in registers, which is at least as accurate as every v
 """
 from __future__ import annotations
 
+import math
+
 import torch
 
 from . import _capi
@@ -408,6 +410,194 @@ def fmha_varlen_fwd(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q: int, m
     _call_on_device(getattr(_capi.lib(), name), args, q.device.index)
 
 
+def kvcache_append(k, v, k_cache, v_cache, cache_seqlens, *, block_table=None, q=None, q_out=None, rotary_cos=None,
+                   rotary_sin=None, rotary_interleaved: bool = False, k_scale: float = 1.0, v_scale: float = 1.0,
+                   seqlens_out=None) -> None:
+    """Append n_new tokens per sequence to a KV cache, with rotary embedding, in one launch on the current CUDA stream of
+    ``k``'s device (``b200_kvcache_append_{f16,bf16}``; with ``block_table``: ``..._paged``).  The write half of
+    FlashAttention's ``flash_attn_with_kvcache`` and vLLM's ``reshape_and_cache_flash``.
+
+    ``k``, ``v`` are ``[B, Hkv, n_new, D]`` fp16 or bf16.  ``cache_seqlens`` (int32 ``[B]``) gives the tokens sequence b
+    already holds, ``L_b = clamp(cache_seqlens[b], 0, capacity)``; new token t goes to position ``L_b + t``.  Dense
+    ``k_cache``, ``v_cache`` are ``[B, Hkv, Nk, D]`` (capacity Nk, the layout ``fmha_fwd(seqlens_k=)`` reads); with
+    ``block_table`` (int32 ``[B, max_pages_per_seq]``) they are pools ``[num_pages, page_size, Hkv, D]`` (capacity
+    ``max_pages_per_seq * page_size``) and position p is row ``p % page_size`` of page ``block_table[b, p // page_size]``.
+    Tokens past capacity, and tokens whose table entry is outside ``[0, num_pages)``, are not written; no other cache
+    byte changes.  Two sequences writing the same row of a shared page race (not detected).
+
+    The cache has k's dtype, or is ``torch.float8_e4m3fn``: then it receives ``(x.float() / scale).clamp(-448, 448)``
+    in e4m3 (round to nearest even), x the fp16 / bf16 value after rotary, k with ``k_scale`` and v with ``v_scale``
+    (finite, > 0; exactly 1 for an fp16 / bf16 cache).
+
+    ``rotary_cos``, ``rotary_sin`` (fp32 ``[rotary_len, rotary_dim / 2]``, ``rotary_len >= capacity + n_new``,
+    ``rotary_dim`` a multiple of 16 up to D) rotate k (never v) at each token's position: pair i is ``(2i, 2i+1)`` with
+    ``rotary_interleaved`` (GPT-J) and ``(i, i + rotary_dim / 2)`` without (NeoX / Llama), ``x0' = x0 cos - x1 sin``,
+    ``x1' = x0 sin + x1 cos`` in fp32, rounded once; columns past rotary_dim are copied.  ``q`` (``[B, H, n_new, D]``) is
+    rotated at the same positions into ``q_out`` (default: ``q`` itself, in place; otherwise a tensor that shares no
+    memory with the others).  ``seqlens_out`` (int32 ``[B]``, not ``cache_seqlens``) receives ``min(L_b + n_new,
+    capacity)``, the ``seqlens_k`` of the attention call.  Lengths and tables are read on the GPU only (no host
+    synchronisation), so a captured CUDA graph replays with the values the tensors hold."""
+    who = "leetcuda_b200.flash_attn.kvcache_append"
+    _append(who, k, v, k_cache, v_cache, cache_seqlens, block_table, q, q_out, rotary_cos, rotary_sin,
+            rotary_interleaved, k_scale, v_scale, seqlens_out)
+
+
+def _append(who, k, v, k_cache, v_cache, cache_seqlens, block_table, q, q_out, rotary_cos, rotary_sin,
+            rotary_interleaved, k_scale, v_scale, seqlens_out) -> None:
+    named = (("k", k), ("v", v), ("k_cache", k_cache), ("v_cache", v_cache), ("cache_seqlens", cache_seqlens))
+    opt = (("block_table", block_table), ("q", q), ("q_out", q_out), ("rotary_cos", rotary_cos),
+           ("rotary_sin", rotary_sin), ("seqlens_out", seqlens_out))
+    for name, t in named + opt:
+        if (t is not None or name in dict(named)) and not isinstance(t, torch.Tensor):
+            raise RuntimeError(f"{who}: {name} must be a torch.Tensor")
+    if q_out is not None and q is None:
+        raise RuntimeError(f"{who}: q_out needs q")
+    if (rotary_cos is None) != (rotary_sin is None):
+        raise RuntimeError(f"{who}: rotary_cos and rotary_sin must both be given or both be None")
+    if k.dtype not in (torch.float16, torch.bfloat16) or v.dtype != k.dtype:
+        raise RuntimeError(f"{who}: k and v must share one dtype, fp16 or bf16, got k {k.dtype}, v {v.dtype}"
+                           .replace("torch.", ""))
+    if k_cache.dtype != v_cache.dtype or k_cache.dtype not in (k.dtype, torch.float8_e4m3fn):
+        raise RuntimeError(f"{who}: k_cache and v_cache must both have k's dtype or both be float8_e4m3fn, got "
+                           f"k_cache {k_cache.dtype}, v_cache {v_cache.dtype} with k {k.dtype}".replace("torch.", ""))
+    e4m3 = k_cache.dtype == torch.float8_e4m3fn
+    if k.dim() != 4 or tuple(v.shape) != tuple(k.shape):
+        raise RuntimeError(f"{who}: k and v must be [B, Hkv, n_new, D] of one shape, got k {tuple(k.shape)}, "
+                           f"v {tuple(v.shape)}")
+    B, Hkv, n_new, D = k.shape
+    paged = block_table is not None
+    if paged:
+        if k_cache.dim() != 4 or tuple(v_cache.shape) != tuple(k_cache.shape) or tuple(k_cache.shape[2:]) != (Hkv, D):
+            raise RuntimeError(f"{who}: with block_table, k_cache and v_cache must be pools [num_pages, page_size, Hkv, "
+                               f"D] of one shape with Hkv = {Hkv}, D = {D}, got k_cache {tuple(k_cache.shape)}, "
+                               f"v_cache {tuple(v_cache.shape)}")
+        num_pages, page_size = k_cache.shape[:2]
+        if page_size < 16 or page_size & (page_size - 1):
+            raise RuntimeError(f"{who}: page_size (k_cache.shape[1]) must be a power of two >= 16, got {page_size}")
+        t = block_table
+        if t.dtype != torch.int32 or t.dim() != 2 or t.shape[0] != B or t.shape[1] < 1:
+            raise RuntimeError(f"{who}: block_table must be an int32 contiguous CUDA tensor [B, max_pages_per_seq] = "
+                               f"[{B}, >= 1] on k's device")
+        capacity = t.shape[1] * page_size
+    else:
+        if k_cache.dim() != 4 or tuple(v_cache.shape) != tuple(k_cache.shape) or k_cache.shape[0] != B \
+                or k_cache.shape[1] != Hkv or k_cache.shape[3] != D:
+            raise RuntimeError(f"{who}: k_cache and v_cache must be [B, Hkv, Nk, D] of one shape with B = {B}, "
+                               f"Hkv = {Hkv}, D = {D}, got k_cache {tuple(k_cache.shape)}, v_cache {tuple(v_cache.shape)}")
+        capacity = k_cache.shape[2]
+    H = Hkv
+    if q is not None:
+        if q.dtype != k.dtype or q.dim() != 4 or q.shape[0] != B or q.shape[2] != n_new or q.shape[3] != D \
+                or q.shape[1] < 1 or q.shape[1] % max(Hkv, 1):
+            raise RuntimeError(f"{who}: q must be [B, H, n_new, D] = [{B}, H, {n_new}, {D}] of k's dtype with Hkv = "
+                               f"{Hkv} dividing H, got {tuple(q.shape)} {q.dtype}".replace("torch.", ""))
+        H = q.shape[1]
+        if q_out is None:
+            q_out = q
+        elif q_out.dtype != q.dtype or tuple(q_out.shape) != tuple(q.shape):
+            raise RuntimeError(f"{who}: q_out must have q's shape and dtype")
+    rotary_dim = rotary_len = 0
+    if rotary_cos is not None:
+        c, s = rotary_cos, rotary_sin
+        if c.dtype != torch.float32 or s.dtype != torch.float32 or c.dim() != 2 or tuple(s.shape) != tuple(c.shape):
+            raise RuntimeError(f"{who}: rotary_cos and rotary_sin must be fp32 [rotary_len, rotary_dim / 2] of one shape")
+        rotary_len, rotary_dim = c.shape[0], 2 * c.shape[1]
+        if rotary_dim < 16 or rotary_dim > D or rotary_dim % 16:
+            raise RuntimeError(f"{who}: rotary_dim = 2 * rotary_cos.shape[1] = {rotary_dim} must be a multiple of 16 in "
+                               f"16 .. D = {D}")
+        if rotary_len < capacity + n_new:
+            raise RuntimeError(f"{who}: rotary_cos.shape[0] = {rotary_len} must be >= capacity + n_new = "
+                               f"{capacity + n_new} (the largest position a token can get, plus one)")
+    elif rotary_interleaved:
+        raise RuntimeError(f"{who}: rotary_interleaved needs rotary_cos and rotary_sin")
+    for name, x in (("k_scale", k_scale), ("v_scale", v_scale)):
+        x = float(x)
+        if not (math.isfinite(x) and x > 0):
+            raise RuntimeError(f"{who}: {name}={x!r} must be finite and > 0")
+        if not e4m3 and x != 1.0:
+            raise RuntimeError(f"{who}: {name}={x!r} must be 1 unless the cache is float8_e4m3fn")
+    for name, t in (("cache_seqlens", cache_seqlens), ("seqlens_out", seqlens_out)):
+        if t is not None and (t.dtype != torch.int32 or tuple(t.shape) != (B,)):
+            raise RuntimeError(f"{who}: {name} must be an int32 contiguous CUDA tensor [B] = [{B}] on k's device")
+    present = [(n, t) for n, t in named + opt if t is not None]
+    for name, t in present:
+        if not t.is_cuda or t.device != k.device:
+            raise RuntimeError(f"{who}: {name} must be a CUDA tensor on k's device (no CPU path)")
+        if not t.is_contiguous():
+            raise RuntimeError(f"{who}: {name} must be contiguous")
+    # every buffer the kernel writes shares no byte with another one; q_out may be q itself (rotated in place)
+    present = [(n, t) for n, t in present if n != "q_out" and t is not None]
+    if q_out is not None and q_out.data_ptr() != q.data_ptr():
+        present.append(("q_out", q_out))
+    for wname, w in present:
+        if wname in ("k_cache", "v_cache", "q_out", "seqlens_out"):
+            for name, t in present:
+                if name != wname and _capi.overlaps(w, t):
+                    raise RuntimeError(f"{who}: {wname} overlaps {name}")
+    ptr = lambda t: None if t is None else t.data_ptr()   # noqa: E731
+    cdt = _capi.DTYPE_E4M3 if e4m3 else (_capi.DTYPE_BF16 if k.dtype == torch.bfloat16 else _capi.DTYPE_F16)
+    name = "b200_kvcache_append_bf16" if k.dtype == torch.bfloat16 else "b200_kvcache_append_f16"
+    head = [k.data_ptr(), v.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr()]
+    mid = [cache_seqlens.data_ptr(), ptr(seqlens_out), ptr(q), ptr(q_out), ptr(rotary_cos), ptr(rotary_sin), B, H, Hkv,
+           n_new]
+    tail = [D, rotary_dim, rotary_len, int(bool(rotary_interleaved)), cdt, float(k_scale), float(v_scale)]
+    if paged:
+        args = head + [block_table.data_ptr()] + mid + [num_pages, page_size, block_table.shape[1]] + tail
+        name += "_paged"
+    else:
+        args = head + mid + [capacity] + tail
+    idx = k.device.index
+    if torch.cuda.current_device() != idx:
+        with torch.cuda.device(idx):
+            rc = getattr(_capi.lib(), name)(*args, _capi.raw_stream(idx))
+    else:
+        rc = getattr(_capi.lib(), name)(*args, _capi.raw_stream(idx))
+    _capi.check(rc, "kvcache_append")
+
+
+def fmha_fwd_kvcache(q, k_cache, v_cache, o, k, v, cache_seqlens, *, block_table=None, rotary_cos=None,
+                     rotary_sin=None, rotary_interleaved: bool = False, causal: bool = False, scale: float = 0.0,
+                     lse=None, num_splits: int = 1, k_scale: float = 1.0, v_scale: float = 1.0):
+    """One decode or chunked-prefill step: append ``k``, ``v`` (``[B, Hkv, n_new, D]``) to the cache with
+    ``kvcache_append`` (rotary on q and k at positions ``L_b + t``, e4m3 quantisation for a ``float8_e4m3fn`` cache,
+    paging through ``block_table``), then attend ``q`` (``[B, H, n_new, D]``) over the cache with ``fmha_fwd``
+    (``seqlens_k`` = the new lengths, ``seqlens_q`` = None so Nq = n_new, ``block_table``, ``k_scale`` / ``v_scale``),
+    writing ``o``.  Returns the new lengths, int32 ``[B]``: ``min(L_b + n_new, capacity)``.
+
+    The queries are the last n_new positions of each sequence, which is where the causal diagonal sits (bottom-right),
+    and q is rotated at the same positions ``L_b + t`` as the keys, causal or not.  FlashAttention's
+    ``flash_attn_with_kvcache`` rotates non-causal q at ``L_b`` for every t instead; with n_new = 1 the two agree.
+    The rotated q goes into a new tensor (``q`` is not modified); without rotary tables ``q`` is used as it is.
+    Two launches plus the attention's split combine if any (1 + 1 or 2).  ``k`` and ``v`` are required: attention over a
+    cache without an append is ``fmha_fwd(seqlens_k=)``.  Everything is read on the GPU, with no host synchronisation,
+    so the step can be captured in a CUDA graph."""
+    who = "leetcuda_b200.flash_attn.fmha_fwd_kvcache"
+    for name, t in (("q", q), ("o", o), ("k", k), ("v", v)):
+        if not isinstance(t, torch.Tensor):
+            raise RuntimeError(f"{who}: {name} must be a torch.Tensor (k and v are required)")
+    if q.dim() != 4 or tuple(o.shape) != tuple(q.shape) or o.dtype != q.dtype:
+        raise RuntimeError(f"{who}: o must have q's shape [B, H, n_new, D] and dtype")
+    if q.shape[3] > 1024:
+        raise RuntimeError(f"{who}: headdim not support! (D={q.shape[3]} > 1024)")
+    if k.dim() != 4 or q.dtype != k.dtype or (q.shape[0], q.shape[2], q.shape[3]) != (k.shape[0], k.shape[2], k.shape[3]) \
+            or k.shape[1] < 1 or q.shape[1] % k.shape[1]:
+        raise RuntimeError(f"{who}: q must be [B, H, n_new, D] of k's dtype, k [B, Hkv, n_new, D] with Hkv dividing H, "
+                           f"got q {tuple(q.shape)} {q.dtype}, k {tuple(k.shape)} {k.dtype}".replace("torch.", ""))
+    _check_lengths(q, q.shape[0], q.shape[1], q.shape[2], num_splits, lse, None, None)
+    if isinstance(cache_seqlens, torch.Tensor) and cache_seqlens.dim() == 1:
+        new_lens = torch.empty(cache_seqlens.shape[0], dtype=torch.int32, device=cache_seqlens.device)
+    else:
+        new_lens = None   # _append rejects it
+    q_rot = torch.empty_like(q) if rotary_cos is not None else None
+    _append(who, k, v, k_cache, v_cache, cache_seqlens, block_table, None if q_rot is None else q, q_rot, rotary_cos,
+            rotary_sin, rotary_interleaved, k_scale, v_scale, new_lens)
+    kw = dict(scale=scale, lse=lse, causal=causal, num_splits=num_splits, seqlens_k=new_lens, block_table=block_table)
+    if k_cache.dtype == torch.float8_e4m3fn:
+        kw.update(k_scale=k_scale, v_scale=v_scale)
+    fmha_fwd(q if q_rot is None else q_rot, k_cache, v_cache, o, **kw)
+    return new_lens
+
+
 def _call_on_device(fn, args, idx) -> None:
     if torch.cuda.current_device() != idx:
         with torch.cuda.device(idx):
@@ -494,4 +684,5 @@ def flash_attn_cute(Q, K, V, O) -> None:
     _fmha_one_length(Q, K, V, O)
 
 
-__all__ = OP_NAMES + ["flash_attn_cute", "fmha_fwd", "fmha_varlen_fwd", "fmha_host", "OP_NAMES", "V_TRANSPOSED_OPS"]
+__all__ = OP_NAMES + ["flash_attn_cute", "fmha_fwd", "fmha_varlen_fwd", "fmha_host", "kvcache_append",
+           "fmha_fwd_kvcache", "OP_NAMES", "V_TRANSPOSED_OPS"]

@@ -398,6 +398,32 @@ int b200_sgemm_3xtf32(const float* a, const float* b, float* c, int M, int N, in
 /* x[i] <- tf32(x[i]) (round to nearest, ties away), in place, n elements; x 16-byte aligned. */
 int b200_tf32_round_inplace(float* x, size_t n, void* stream);
 
+/* ------------------------------------------------------------------ fp8 (e4m3) scaled GEMM
+ * C[M,N] = OutT( scaled( A[M,K] B[N,K]^T ) ): A and B OCP e4m3 (torch.float8_e4m3fn), both K-major; C fp16 or bf16
+ * (c_dtype B200_DTYPE_F16 / B200_DTYPE_BF16), row-major, written in place.  The layout of torch's _scaled_mm with a
+ * column-major [K,N] b, i.e. a [N,K] row-major weight.
+ *
+ * Accumulation is fp32 with promotion once per 128-element k-block: the tensor core sums each k-block's 128 products on
+ * its own (its internal precision inside a k-block is undocumented), and the kernel adds that partial into fp32
+ * registers.  There is no fast-accumulation mode.  C is rounded once to OutT (round to nearest even; fp16 overflow
+ * gives +-inf).  Scales are fp32 in device memory, read by the kernel only (a captured CUDA graph replays with the
+ * values they hold at replay time):
+ *   B200_SCALE_TENSOR  scale_a[0], scale_b[0]                         C = OutT((acc * scale_a[0]) * scale_b[0])
+ *   B200_SCALE_ROW     scale_a[M], scale_b[N]                          C = OutT((acc[m,n] * scale_a[m]) * scale_b[n])
+ *   B200_SCALE_BLOCK   scale_a [M, ceil(K/128)], M-major (element (m, kb) at m + kb * M, DeepGEMM's layout);
+ *                      scale_b [ceil(N/128), ceil(K/128)], row-major (element (nb, kb) at nb * ceil(K/128) + kb).
+ *                      Every k-block kb is promoted as acc = fma(partial, fp32(scale_a[m,kb] * scale_b[n/128,kb]), acc)
+ *                      and C = OutT(acc) (DeepSeek-V3's 1 x 128 activation and 128 x 128 weight scales).
+ * Constraints (B200_EINVAL, message naming the argument, before any CUDA call): a, b_nk, c, scale_a, scale_b not NULL;
+ * a, b_nk, c 16-byte aligned, the scales 4-byte aligned; M, N, K >= 1; K % 16 == 0 (the TMA row stride); N % 8 == 0
+ * (16-byte C stores); scale_recipe and c_dtype as above; c disjoint from a, b_nk and the scales.  Any M >= 1 and ragged
+ * N and K are handled (k past K is zero-filled).  One launch, no workspace. */
+#define B200_SCALE_TENSOR 0
+#define B200_SCALE_ROW 1
+#define B200_SCALE_BLOCK 2
+int b200_gemm_e4m3(const void* a, const void* b_nk, void* c, const float* scale_a, const float* scale_b, int M, int N,
+                   int K, int scale_recipe, int c_dtype, void* stream);
+
 /* ------------------------------------------------------------------ merge_attn_states
  * Combine two partial attention results over disjoint key ranges (split-KV), SURVEY §8f-3.  Replaces
  *   merge_attn_states_cuda(output, output_lse?, prefix_output, prefix_lse, suffix_output, suffix_lse)
@@ -414,7 +440,8 @@ int b200_tf32_round_inplace(float* x, size_t n, void* stream);
 #define B200_DTYPE_F32 0
 #define B200_DTYPE_F16 1
 #define B200_DTYPE_BF16 2
-#define B200_DTYPE_E4M3 3 /* OCP e4m3 (torch.float8_e4m3fn): KV caches of b200_kvcache_append_* only */
+#define B200_DTYPE_E4M3 3 /* OCP e4m3 (torch.float8_e4m3fn): KV caches of b200_kvcache_append_*; the e4m3 operands
+                            * of b200_gemm_e4m3 have no dtype argument */
 int b200_merge_attn_states(void* output, float* output_lse, const void* prefix_output,
                            const float* prefix_lse, const void* suffix_output, const float* suffix_lse,
                            int num_tokens, int num_heads, int head_size, int dtype, void* stream);

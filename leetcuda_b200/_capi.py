@@ -21,6 +21,7 @@ B_ROW_MAJOR_KN = 0  # "NN"
 B_ROW_MAJOR_NK = 1  # "TN"
 FMHA_MAX_SPLITS = 64  # B200_FMHA_MAX_SPLITS
 DTYPE_F16, DTYPE_BF16, DTYPE_E4M3 = 1, 2, 3  # B200_DTYPE_*
+SCALE_TENSOR, SCALE_ROW, SCALE_BLOCK = 0, 1, 2  # B200_SCALE_*
 
 _lib = None
 
@@ -77,6 +78,7 @@ SIGNATURES = {
     "b200_sgemm_tf32": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200_sgemm_3xtf32": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
     "b200_tf32_round_inplace": (_i, [_vp, ctypes.c_size_t, _vp]),
+    "b200_gemm_e4m3": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200_merge_attn_states": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200_hgemm_f16_host": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200_fmha_fwd_f16_host": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),

@@ -20,7 +20,8 @@ OBJ = HERE / "_build"
 LIB = HERE / "libleetcuda_b200.so"
 
 SOURCES = ["capi_common.cu", "hgemm_capi.cu", "attn_capi.cu", "attn_bf16.cu", "attn_fp8kv_f16.cu", "attn_fp8kv_bf16.cu",
-           "attn_varlen.cu", "merge_capi.cu", "elementwise_capi.cu", "kvcache_capi.cu"]
+           "attn_varlen.cu", "merge_capi.cu", "elementwise_capi.cu", "kvcache_capi.cu",
+           "gemm_fp8_capi.cu"]
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3", "-lineinfo",

@@ -134,6 +134,99 @@ def hgemm_host(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, *, tn: bool = 
     _capi.check(rc, "hgemm_host")
 
 
+SCALE_RECIPES = {"tensor": _capi.SCALE_TENSOR, "row": _capi.SCALE_ROW, "block": _capi.SCALE_BLOCK}
+
+
+def scaled_mm(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor, *,
+              scale_recipe: str, bias=None) -> None:
+    """``c[M,N] = c.dtype(scaled(a @ b))`` for e4m3 operands (``b200_gemm_e4m3``), on the current CUDA stream of
+    ``a``'s device.
+
+    ``a`` is ``[M,K]`` ``torch.float8_e4m3fn``, contiguous.  ``b`` is ``[K,N]`` ``float8_e4m3fn`` in column-major
+    layout (``b.t().is_contiguous()``), torch's ``_scaled_mm`` convention: ``scaled_mm(x, w.t(), ...)`` takes a
+    ``[N,K]`` weight as it is stored.  ``c`` is ``[M,N]`` fp16 or bf16, contiguous, and is written in place.
+    Accumulation is fp32, promoted once per 128-element k-block; C is rounded once.  Scales are fp32 on ``a``'s device
+    and are read by the kernel only, so the call can be captured in a CUDA graph and replayed after new scale values
+    are written.  ``scale_recipe`` says how to read them (scale shapes alone are ambiguous):
+
+    ``"tensor"``  one value each (any shape with one element): ``c = (acc * scale_a) * scale_b``
+    ``"row"``     ``scale_a`` ``[M]`` or ``[M,1]``, ``scale_b`` ``[N]`` or ``[1,N]``, contiguous:
+                  ``c[m,n] = (acc[m,n] * scale_a[m]) * scale_b[n]``
+    ``"block"``   ``scale_a`` ``[M, ceil(K/128)]`` with stride ``(1, M)`` (M-major, DeepGEMM's layout);
+                  ``scale_b`` ``[ceil(N/128), ceil(K/128)]`` row-major (or its transpose ``[ceil(K/128),
+                  ceil(N/128)]`` viewed over the same storage).  Each k-block is promoted as
+                  ``acc = fma(partial, scale_a[m,kb] * scale_b[n//128,kb], acc)``.
+
+    Constraints: K % 16 == 0 and N % 8 == 0.  e5m2 operands, fp32 output and bias are not supported.
+    """
+    def tensor(x, name):
+        if not isinstance(x, torch.Tensor):
+            raise RuntimeError(f"scaled_mm: {name} must be a torch.Tensor")
+    for x, name in ((a, "a"), (b, "b"), (c, "c"), (scale_a, "scale_a"), (scale_b, "scale_b")):
+        tensor(x, name)
+    if bias is not None:
+        raise RuntimeError("scaled_mm: bias is not supported")
+    if scale_recipe not in SCALE_RECIPES:
+        raise RuntimeError(f"scaled_mm: scale_recipe must be 'tensor', 'row' or 'block', got {scale_recipe!r}")
+    for x, name in ((a, "a"), (b, "b")):
+        if x.dtype != torch.float8_e4m3fn:
+            raise RuntimeError(f"scaled_mm: {name} must be torch.float8_e4m3fn (e4m3), got {x.dtype}; e5m2 and other "
+                               "fp8 formats are not supported")
+    if c.dtype not in (torch.float16, torch.bfloat16):
+        raise RuntimeError(f"scaled_mm: c must be torch.float16 or torch.bfloat16, got {c.dtype}")
+    if a.dim() != 2 or b.dim() != 2 or c.dim() != 2:
+        raise RuntimeError("scaled_mm: a, b and c must be 2-D ([M,K], [K,N], [M,N])")
+    M, K = a.shape
+    N = b.shape[1]
+    if b.shape[0] != K or tuple(c.shape) != (M, N):
+        raise RuntimeError(f"scaled_mm: shapes a {tuple(a.shape)}, b {tuple(b.shape)}, c {tuple(c.shape)} do not "
+                           "form [M,K] x [K,N] -> [M,N]")
+    if not a.is_contiguous():
+        raise RuntimeError("scaled_mm: a must be contiguous (row-major [M,K])")
+    if not b.t().is_contiguous():
+        raise RuntimeError("scaled_mm: b must be column-major ([K,N] with b.t() contiguous, e.g. w.t() of a [N,K] "
+                           "weight)")
+    if not c.is_contiguous():
+        raise RuntimeError("scaled_mm: c must be contiguous")
+    for x, name in ((scale_a, "scale_a"), (scale_b, "scale_b")):
+        if x.dtype != torch.float32:
+            raise RuntimeError(f"scaled_mm: {name} must be torch.float32, got {x.dtype}")
+    kbs, nbs = -(-K // 128), -(-N // 128)
+    if scale_recipe == "tensor":
+        if scale_a.numel() != 1 or scale_b.numel() != 1:
+            raise RuntimeError("scaled_mm: tensor scaling takes one scale_a and one scale_b value")
+    elif scale_recipe == "row":
+        if tuple(scale_a.shape) not in ((M,), (M, 1)) or not scale_a.is_contiguous():
+            raise RuntimeError(f"scaled_mm: row scaling takes a contiguous scale_a of shape [{M}] or [{M}, 1]")
+        if tuple(scale_b.shape) not in ((N,), (1, N)) or not scale_b.is_contiguous():
+            raise RuntimeError(f"scaled_mm: row scaling takes a contiguous scale_b of shape [{N}] or [1, {N}]")
+    else:
+        if tuple(scale_a.shape) != (M, kbs) or not scale_a.t().is_contiguous():
+            raise RuntimeError(f"scaled_mm: block scaling takes scale_a [{M}, {kbs}] with stride (1, {M}) (M-major)")
+        if not ((tuple(scale_b.shape) == (nbs, kbs) and scale_b.is_contiguous())
+                or (tuple(scale_b.shape) == (kbs, nbs) and scale_b.t().is_contiguous())):
+            raise RuntimeError(f"scaled_mm: block scaling takes scale_b [{nbs}, {kbs}] row-major (or its transpose "
+                               "over the same storage)")
+    for x, name in ((a, "a"), (b, "b"), (scale_a, "scale_a"), (scale_b, "scale_b")):
+        if _capi.overlaps(c, x):
+            raise RuntimeError(f"scaled_mm: c overlaps {name}")
+    if not a.is_cuda:
+        raise RuntimeError("scaled_mm: a must be a CUDA tensor (no CPU path)")
+    for x, name in ((b, "b"), (c, "c"), (scale_a, "scale_a"), (scale_b, "scale_b")):
+        if x.device != a.device:
+            raise RuntimeError(f"scaled_mm: {name} must be on a's device {a.device}, got {x.device}")
+    idx = a.device.index
+    args = (a.data_ptr(), b.data_ptr(), c.data_ptr(), scale_a.data_ptr(), scale_b.data_ptr(), M, N, K,
+            SCALE_RECIPES[scale_recipe], _capi.DTYPE_F16 if c.dtype == torch.float16 else _capi.DTYPE_BF16)
+    fn = _capi.lib().b200_gemm_e4m3
+    if torch.cuda.current_device() != idx:
+        with torch.cuda.device(idx):
+            rc = fn(*args, _capi.raw_stream(idx))
+    else:
+        rc = fn(*args, _capi.raw_stream(idx))
+    _capi.check(rc, "scaled_mm")
+
+
 def _make_3arg(name: str, tn: bool):
     def op(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor) -> None:
         hgemm(a, b, c, tn=tn)
@@ -190,4 +283,4 @@ def destroy_cublas_handle() -> None:
 
 
 __all__ = OP_NAMES + ["init_cublas_handle", "destroy_cublas_handle", "hgemm", "hgemm_host",
-                      "OP_NAMES"]
+                      "scaled_mm", "OP_NAMES"]

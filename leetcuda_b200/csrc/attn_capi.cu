@@ -15,7 +15,6 @@
 namespace {
 
 using namespace b200;
-using b200::attn::launch_kernel;
 using b200::host::fail;
 
 // Split-KV: the most splits b200_fmha_fwd_f16_gqa accepts (B200_FMHA_MAX_SPLITS); for num_splits = 0 the fewest key
@@ -28,42 +27,23 @@ constexpr int kMaxSplits = 64;
 constexpr int kMinBlocksPerSplit = 4;
 constexpr int kMinBlocksToSplit = 16;
 
-// lens != nullptr: per-sequence lengths, attn_fwd_seqlens_kernel (natural V only); with pages also: paged K/V,
-// attn_fwd_paged_kernel
-template <int kDS, int kBN, int kWG, bool kVT>
-int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const attn::Params& p, int qtiles,
-                int BH, int smem, bool causal, bool packed, int splits, const attn::Lens* lens,
-                const attn::Pages* pages, cudaStream_t stream) {
-  if constexpr (!kVT) {
-    if (lens != nullptr && pages != nullptr) {
-      auto kern = splits > 1 ? (causal ? attn::attn_fwd_paged_kernel<kDS, kBN, kWG, true, true>
-                                       : attn::attn_fwd_paged_kernel<kDS, kBN, kWG, false, true>)
-                             : (causal ? attn::attn_fwd_paged_kernel<kDS, kBN, kWG, true, false>
-                                       : attn::attn_fwd_paged_kernel<kDS, kBN, kWG, false, false>);
-      static int attr_smem[4][64] = {};
-      return launch_kernel(kern, attr_smem[2 * (splits > 1) + causal], p, qtiles, BH, splits, attn::threads<kWG>(),
-                           smem, stream, tq, tk, tv, p, *lens, *pages);
+// The fp16 kernel of family F.  lens != nullptr: per-sequence lengths, attn_fwd_seqlens_kernel (natural V only); with
+// pages also: paged K/V, attn_fwd_paged_kernel
+template <typename F, bool kVT>
+int launch_attn(const attn::Launch& l, bool causal, bool packed, const attn::Lens* lens, const attn::Pages* pages) {
+  constexpr int kDS = F::kDS, kBN = F::kBN, kWG = F::kWG;
+  return attn::with_flags(causal, l.splits > 1, [&](auto c, auto s) {
+    if constexpr (!kVT) {
+      if (lens != nullptr && pages != nullptr)
+        return attn::launch<attn::attn_fwd_paged_kernel<kDS, kBN, kWG, c, s>, kWG>(l, *lens, *pages);
+      if (lens != nullptr) return attn::launch<attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, c, s>, kWG>(l, *lens);
     }
-    if (lens != nullptr) {
-      auto kern = splits > 1 ? (causal ? attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, true, true>
-                                       : attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, false, true>)
-                             : (causal ? attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, true, false>
-                                       : attn::attn_fwd_seqlens_kernel<kDS, kBN, kWG, false, false>);
-      static int attr_smem[4][64] = {};
-      return launch_kernel(kern, attr_smem[2 * (splits > 1) + causal], p, qtiles, BH, splits, attn::threads<kWG>(),
-                           smem, stream, tq, tk, tv, p, *lens);
+    // packed query heads need the kGQA kernels only for the mask; a split always runs a kSplit kernel
+    if constexpr (c && !s) {
+      if (packed) return attn::launch<attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true, true>, kWG>(l);
     }
-  }
-  // packed query heads need the kGQA kernels only for the mask; a split always runs a kSplit kernel
-  auto kern = splits > 1 ? (causal ? attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true, true, true>
-                                   : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, false, false, true>)
-                         : (causal ? (packed ? attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true, true>
-                                             : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, true>)
-                                   : attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, false>);
-  const int variant = splits > 1 ? 3 + causal : causal + (causal && packed);
-  static int attr_smem[5][64] = {};
-  return launch_kernel(kern, attr_smem[variant], p, qtiles, BH, splits, attn::threads<kWG>(), smem, stream, tq, tk, tv,
-                       p);
+    return attn::launch<attn::attn_fwd_kernel<kDS, kBN, kWG, kVT, c, c && s, s>, kWG>(l);
+  });
 }
 
 // [BH, D, N] -> [BH, N, D] (fp16): the three reference ops that take V pre-transposed
@@ -144,18 +124,15 @@ int launch_combine(T* out, float* out_lse, const float* ws_o, const float* ws_ls
   return 0;
 }
 
-// Kernel shape per head dim (attn_sm90.cuh):
-//   D <= 64        one 64-column slab, 128-key blocks, two consumer warpgroups (128 query rows)
-//   64 < D <= 128  one 128-column slab, 64-key blocks, two consumer warpgroups
-//   128 < D        256-column slabs (S recomputed per slab), 64-key blocks, one consumer warpgroup (64 query rows)
-// The S, P and O fragments of a consumer thread have to fit its registers: ptxas gives a 384-thread CTA
-// 168 per thread, a 256-thread CTA 255 (O of a 256-column slab alone takes 128).
+// The family of head dim D (attn::with_family) at run time
 struct Family {
   int ds, bn, wgs;
 };
 Family family(int D) {
-  const int ds = D <= 64 ? 64 : (D <= 128 ? 128 : 256);
-  return {ds, ds == 64 ? 128 : 64, ds == 256 ? 1 : 2};
+  return attn::with_family(D, [](auto f) {
+    using F = decltype(f);
+    return Family{F::kDS, F::kBN, F::kWG};
+  });
 }
 
 // The K/V ring of family f next to Q (nq 64-column chunks per tile row): every slot that fits, at most 16 (two key
@@ -169,6 +146,30 @@ int ring_smem(const Family& f, int nq, bool vt, int stage, int* ring) {
   if (*ring > 16) *ring = 16;
   if (*ring < 2) return 0;
   return attn::smem_bytes(f.wgs, slot, nq, *ring) + *ring * stage;
+}
+
+// *p for G * Nq packed rows per K/V head (Nq query positions per head) against Nk keys on the family of D, without a
+// split workspace and with p->tph = 0, and its K/V ring (ring_smem).  Returns the dynamic shared memory, or 0 when
+// the ring does not fit.
+int attn_params(attn::Params* p, int G, int Nq, int Nk, int D, float scale, float* lse, float rms_g, void* o, bool vt,
+                int stage) {
+  const Family f = family(D);
+  p->Nq = G * Nq;
+  p->qpos = Nq;
+  p->Nk = Nk;
+  p->D = D;
+  p->nq = (D + 63) / 64;
+  p->num_kv = (Nk + f.bn - 1) / f.bn;
+  p->diag = Nk - Nq;
+  p->slabs = (D + f.ds - 1) / f.ds;
+  p->scale_log2 = scale * 1.4426950408889634f;
+  p->lse = lse;
+  p->rms_g = rms_g;
+  p->o_ptr = static_cast<__half*>(o);
+  p->ws_o = nullptr;
+  p->ws_lse = nullptr;
+  p->tph = 0;
+  return ring_smem(f, p->nq, vt, stage, &p->ring);
 }
 
 // A tensor map over `rows` rows of `heads` heads of D elements (row-major [rows, heads, D]): dims {D, heads, rows},
@@ -198,26 +199,14 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
   const Family f = family(D);
   const int ds = f.ds, bn = f.bn, wgs = f.wgs;
   const int rows = G * Nq;   // packed rows per K/V head
-  attn::Params p;
-  p.Nq = rows;
-  p.qpos = Nq;
-  p.Nk = Nk;
-  p.D = D;
-  p.nq = (D + 63) / 64;
-  p.num_kv = (Nk + bn - 1) / bn;
-  p.diag = Nk - Nq;
-  p.slabs = (D + ds - 1) / ds;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  p.lse = lse;
-  p.rms_g = rms_g;
-  p.o_ptr = static_cast<__half*>(o);
-  p.ws_o = splits > 1 ? ws_o : nullptr;
-  p.ws_lse = splits > 1 ? ws_lse : nullptr;
   if (rms_g > 0.f && D > 256 && !(D <= 512 && D % 128 == 0))
     return fail(B200_ENOTSUP, "fused rms_norm: D=%d (supported: D <= 256, 384, 512)", D);
+  attn::Params p;
   // fp8: every ring slot has a staging chunk of e4m3 bytes and its barrier beside it (attn_sm90.cuh)
-  const int smem = ring_smem(f, p.nq, vt, fp8 ? 64 * bn + 8 : 0, &p.ring);
+  const int smem = attn_params(&p, G, Nq, Nk, D, scale, lse, rms_g, o, vt, fp8 ? 64 * bn + 8 : 0);
   if (smem == 0) return fail(B200_ENOTSUP, "headdim not support! (D=%d)", D);
+  p.ws_o = splits > 1 ? ws_o : nullptr;
+  p.ws_lse = splits > 1 ? ws_lse : nullptr;
   // causal packed heads of at least one tile of rows: tiles of their own per head (attn_sm90.cuh), else packed tiles
   p.tph = causal && Nq >= 64 * wgs ? (Nq + 64 * wgs - 1) / (64 * wgs) : 0;
   const int qtiles = p.tph > 0 ? G * p.tph : (rows + 64 * wgs - 1) / (64 * wgs);
@@ -254,32 +243,24 @@ int fmha_dispatch(const void* q, const void* k, const void* v, void* o, float* l
       if ((rc = host::get_tmap(&tv, v, 3, kdims, kstr, kbox, kvsw, kvdt))) return rc;
     }
   }
-  const int bh = static_cast<int>(BH);
   if (vt && lens) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with lengths)");
-  const bool pk = G > 1;
-  const attn::Pages* pg = pages;
+  const attn::Launch l{tq, tk, tv, p, qtiles, static_cast<int>(BH), splits, smem, stream};
   if constexpr (fp8) {
     if (vt || !lens) return fail(B200_EINVAL, "fmha: internal dispatch error (fp8 K/V without lengths or with V^T)");
-    if (ds == 64)
-      return attn::launch_attn_fp8kv<T, 64, 128, 2>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, v_scale,
-                                                    stream);
-    if (ds == 128)
-      return attn::launch_attn_fp8kv<T, 128, 64, 2>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, v_scale,
-                                                    stream);
-    return attn::launch_attn_fp8kv<T, 256, 64, 1>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, v_scale,
-                                                  stream);
+    return attn::launch_attn_fp8kv<T>(l, causal, *lens, pages, v_scale);
   } else if constexpr (bf16) {
     if (vt || !lens) return fail(B200_EINVAL, "fmha: internal dispatch error (bf16 without lengths or with V^T)");
-    if (ds == 64) return attn::launch_attn_bf16<64, 128, 2>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, stream);
-    if (ds == 128) return attn::launch_attn_bf16<128, 64, 2>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, stream);
-    return attn::launch_attn_bf16<256, 64, 1>(tq, tk, tv, p, qtiles, bh, smem, causal, splits, *lens, pg, stream);
+    return attn::launch_attn_bf16(l, causal, *lens, pages);
+  } else {
+    return attn::with_family(D, [&](auto fam) {
+      using F = decltype(fam);
+      if (!vt) return launch_attn<F, false>(l, causal, G > 1, lens, pages);
+      if constexpr (F::kDS == 256)
+        return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with D=%d)", D);
+      else
+        return launch_attn<F, true>(l, causal, G > 1, lens, pages);
+    });
   }
-  if (ds == 64) return vt ? launch_attn<64, 128, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream)
-                          : launch_attn<64, 128, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream);
-  if (ds == 128) return vt ? launch_attn<128, 64, 2, true>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream)
-                           : launch_attn<128, 64, 2, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream);
-  if (vt) return fail(B200_EINVAL, "fmha: internal dispatch error (transposed V with D=%d)", D);
-  return launch_attn<256, 64, 1, false>(tq, tk, tv, p, qtiles, bh, smem, causal, pk, splits, lens, pg, stream);
 }
 
 // The attention kernel, and with splits > 1 its fp32 parts in a stream-ordered workspace and the combine kernel.
@@ -308,14 +289,7 @@ int fmha_run(const void* q, const void* k, const void* v, void* o, float* lse, f
 // would not finish sooner), keeping at least kMinBlocksPerSplit key blocks per split; 1 when the grid already fills
 // the machine or the keys span fewer than kMinBlocksToSplit blocks.
 int auto_splits(int B, int Hkv, int G, int Nq, int Nk, int D) {
-  static int sms[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  int n = dev >= 0 && dev < 64 ? sms[dev] : 0;
-  if (n == 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 1;
-    if (dev >= 0 && dev < 64) sms[dev] = n;
-  }
+  const int n = host::sm_count();
   const Family f = family(D);
   const long long rows = static_cast<long long>(G) * Nq;
   const long long ctas = (rows + 64 * f.wgs - 1) / (64 * f.wgs) * ((D + f.ds - 1) / f.ds) * B * Hkv;
@@ -325,6 +299,79 @@ int auto_splits(int B, int Hkv, int G, int Nq, int Nk, int D) {
   s = std::min<long long>(s, num_kv / kMinBlocksPerSplit);
   s = std::min<long long>(s, kMaxSplits);
   return s < 1 ? 1 : static_cast<int>(s);
+}
+
+// The argument checks the attention entries share: each returns 0 or fails with a message that starts with the
+// entry's name (who).
+
+// b200_fmha_fwd_f16_kv and _gqa: both lengths, the causal flag, and Nk % 8 for transposed V
+int check_kv(const char* who, int Nq, int Nk, int v_transposed, int causal) {
+  if (Nq <= 0 || Nk <= 0) return fail(B200_EINVAL, "%s: bad lengths Nq=%d Nk=%d (both must be >= 1)", who, Nq, Nk);
+  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "%s: causal must be 0 or 1, got %d", who, causal);
+  if (v_transposed && (Nk % 8) != 0)
+    return fail(B200_EINVAL, "%s: Nk (%d) must be a multiple of 8 for transposed V", who, Nk);
+  return 0;
+}
+
+int check_hkv(const char* who, int H, int Hkv) {
+  if (Hkv <= 0 || H % Hkv != 0) return fail(B200_EINVAL, "%s: Hkv=%d must be >= 1 and divide H=%d", who, Hkv, H);
+  return 0;
+}
+
+// grid.y: B * Hkv K/V heads (heads names the product: "B*Hkv", or "B*H" where every head has its own K/V head)
+int check_grid_heads(const char* who, const char* heads, int B, int Hkv) {
+  if (static_cast<long long>(B) * Hkv > 65535)
+    return fail(B200_EINVAL, "%s: %s = %lld exceeds the grid limit 65535", who, heads, static_cast<long long>(B) * Hkv);
+  return 0;
+}
+
+int check_splits(const char* who, int num_splits) {
+  if (num_splits < 0 || num_splits > kMaxSplits)
+    return fail(B200_EINVAL, "%s: num_splits=%d must be in 0 .. %d", who, num_splits, kMaxSplits);
+  return 0;
+}
+
+int check_split_out(const char* who, int num_splits, const void* o) {
+  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
+    return fail(B200_EINVAL, "%s: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)", who);
+  return 0;
+}
+
+// G * nq packed query rows per K/V head; nq_name: "Nq" or "max_seqlen_q"
+int check_rows(const char* who, int G, int nq, const char* nq_name) {
+  if (static_cast<long long>(G) * nq > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "%s: (H/Hkv)*%s = %lld query rows per K/V head exceed 2^31 - 1", who, nq_name,
+                static_cast<long long>(G) * nq);
+  return 0;
+}
+
+int check_int32(const char* who, const int* a, const char* name) {
+  if ((reinterpret_cast<uintptr_t>(a) & 3u) != 0)
+    return fail(B200_EINVAL, "%s: %s must be 4-byte aligned (int32)", who, name);
+  return 0;
+}
+
+// a paged K/V pool of num_pages pages of page_size rows, and block tables of max_pages entries
+int check_pool(const char* who, int num_pages, int page_size, int max_pages) {
+  if (num_pages < 1) return fail(B200_EINVAL, "%s: num_pages=%d must be >= 1", who, num_pages);
+  if (max_pages < 1) return fail(B200_EINVAL, "%s: max_pages_per_seq=%d must be >= 1", who, max_pages);
+  if (page_size < 16 || (page_size & (page_size - 1)) != 0)
+    return fail(B200_EINVAL, "%s: page_size=%d must be a power of two >= 16", who, page_size);
+  if (static_cast<long long>(num_pages) * page_size > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "%s: num_pages*page_size = %lld pool rows exceed 2^31 - 1", who,
+                static_cast<long long>(num_pages) * page_size);
+  if (static_cast<long long>(max_pages) * page_size > 0x7FFFFFFFll)
+    return fail(B200_EINVAL, "%s: max_pages_per_seq*page_size = %lld keys per sequence exceed 2^31 - 1", who,
+                static_cast<long long>(max_pages) * page_size);
+  return 0;
+}
+
+// who = "": the message is the reference's, without a prefix
+int check_head_dim(const char* who, int D) {
+  const char* sep = *who ? ": " : "";
+  if (D % 8 != 0) return fail(B200_ENOTSUP, "%s%sheaddim not support! (D=%d must be a multiple of 8)", who, sep, D);
+  if (D > 1024) return fail(B200_ENOTSUP, "%s%sheaddim not support! (D=%d > 1024)", who, sep, D);
+  return 0;
 }
 
 // The checks common to every attention entry and the transpose pre-pass.  The entries with one sequence length pass
@@ -338,10 +385,8 @@ int fmha_impl(const void* q, const void* k, const void* v, void* o, float* lse, 
   if (B <= 0 || H <= 0 || Nq <= 0 || Nk <= 0 || D <= 0)
     return fail(B200_EINVAL, "fmha: bad shape B=%d H=%d N=%d D=%d", B, H, Nq, D);
   const int Hkv = H / G;
-  if (static_cast<long long>(B) * Hkv > 65535)
-    return fail(B200_EINVAL, "fmha: B*H = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
-  if (D % 8 != 0) return fail(B200_ENOTSUP, "headdim not support! (D=%d must be a multiple of 8)", D);
-  if (D > 1024) return fail(B200_ENOTSUP, "headdim not support! (D=%d > 1024)", D);
+  if (int rc = check_grid_heads("fmha", "B*H", B, Hkv)) return rc;
+  if (int rc = check_head_dim("", D)) return rc;
   if (v_transposed && (Nk % 8) != 0)
     return fail(B200_EINVAL, "fmha: N (%d) must be a multiple of 8 for transposed V", Nk);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -392,100 +437,47 @@ int fp8kv_scales(const char* who, int D, float k_scale, float v_scale, float* sc
   return 0;
 }
 
-// b200_fmha_fwd_{f16,bf16}_seqlens and _paged: the same checks and messages for both element types T, and for the
-// fp8-K/V entries (KV = __nv_fp8_e4m3) with their own checks after these.
+// b200_fmha_fwd_{f16,bf16}_seqlens (pages == nullptr, who "fmha_seqlens") and _paged (who "fmha_paged": k and v are
+// pools of num_pages pages [page_size, Hkv, D] read through pages->table, and Nk is the padded max_pages * page_size):
+// the same checks and messages for both element types T, and for the fp8-K/V entries (KV = __nv_fp8_e4m3) with their
+// own checks after these.
 template <typename T, typename KV = T>
-int fmha_seqlens(const void* q, const void* k, const void* v, void* o, float* lse, const int* seqlens_q,
-                              const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk, int D, int causal,
-                              int num_splits, float scale, void* stream, float k_scale = 1.f, float v_scale = 1.f) {
+int fmha_lens(const void* q, const void* k, const void* v, void* o, float* lse, const int* seqlens_q,
+              const int* seqlens_k, const attn::Pages* pages, int num_pages, int B, int H, int Hkv, int Nq, int Nk,
+              int D, int causal, int num_splits, float scale, void* stream, float k_scale = 1.f, float v_scale = 1.f) {
+  const char* who = pages ? "fmha_paged" : "fmha_seqlens";
+  if (pages && (!q || !k || !v || !o || !pages->table))
+    return fail(B200_EINVAL, "fmha_paged: null pointer (q, k_cache, v_cache, o and block_table are required)");
   if (!q || !k || !v || !o) return fail(B200_EINVAL, "fmha_seqlens: null pointer (q, k, v and o are required)");
-  if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "fmha_seqlens: bad shape B=%d H=%d D=%d", B, H, D);
-  if (Nq <= 0 || Nk <= 0)
+  if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "%s: bad shape B=%d H=%d D=%d", who, B, H, D);
+  if (pages && Nq <= 0) return fail(B200_EINVAL, "fmha_paged: bad length Nq=%d (must be >= 1)", Nq);
+  if (!pages && (Nq <= 0 || Nk <= 0))
     return fail(B200_EINVAL, "fmha_seqlens: bad lengths Nq=%d Nk=%d (both must be >= 1)", Nq, Nk);
-  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_seqlens: causal must be 0 or 1, got %d", causal);
-  if (Hkv <= 0 || H % Hkv != 0)
-    return fail(B200_EINVAL, "fmha_seqlens: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
-  if (num_splits < 0 || num_splits > kMaxSplits)
-    return fail(B200_EINVAL, "fmha_seqlens: num_splits=%d must be in 0 .. %d", num_splits, kMaxSplits);
-  if (static_cast<long long>(B) * Hkv > 65535)
-    return fail(B200_EINVAL, "fmha_seqlens: B*Hkv = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
-  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
-    return fail(B200_EINVAL,
-                "fmha_seqlens: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)");
-  if (static_cast<long long>(H / Hkv) * Nq > 0x7FFFFFFFll)
-    return fail(B200_EINVAL, "fmha_seqlens: (H/Hkv)*Nq = %lld query rows per K/V head exceed 2^31 - 1",
-                static_cast<long long>(H / Hkv) * Nq);
-  if ((reinterpret_cast<uintptr_t>(seqlens_q) & 3u) != 0)
-    return fail(B200_EINVAL, "fmha_seqlens: seqlens_q must be 4-byte aligned (int32)");
-  if ((reinterpret_cast<uintptr_t>(seqlens_k) & 3u) != 0)
-    return fail(B200_EINVAL, "fmha_seqlens: seqlens_k must be 4-byte aligned (int32)");
-  if (D % 8 != 0) return fail(B200_ENOTSUP, "fmha_seqlens: headdim not support! (D=%d must be a multiple of 8)", D);
-  if (D > 1024) return fail(B200_ENOTSUP, "fmha_seqlens: headdim not support! (D=%d > 1024)", D);
+  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "%s: causal must be 0 or 1, got %d", who, causal);
+  if (int rc = check_hkv(who, H, Hkv)) return rc;
+  if (int rc = check_splits(who, num_splits)) return rc;
+  if (int rc = check_grid_heads(who, "B*Hkv", B, Hkv)) return rc;
+  if (int rc = check_split_out(who, num_splits, o)) return rc;
+  if (int rc = check_rows(who, H / Hkv, Nq, "Nq")) return rc;
+  if (int rc = check_int32(who, seqlens_q, "seqlens_q")) return rc;
+  if (int rc = check_int32(who, seqlens_k, "seqlens_k")) return rc;
+  if (pages) {
+    if (int rc = check_int32(who, pages->table, "block_table")) return rc;
+    if (int rc = check_pool(who, num_pages, pages->page_size, pages->max_pages)) return rc;
+    Nk = pages->max_pages * pages->page_size;
+  }
+  if (int rc = check_head_dim(who, D)) return rc;
   if constexpr (!std::is_same_v<KV, T>) {
-    if (int rc = fp8kv_scales("fmha_seqlens", D, k_scale, v_scale, &scale)) return rc;
+    if (int rc = fp8kv_scales(who, D, k_scale, v_scale, &scale)) return rc;
   }
   if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
   const int G = H / Hkv;
   // the split count follows the padded shape, as for b200_fmha_fwd_f16_gqa: the lengths stay on the device (and
-  // b200_fmha_fwd_f16_gqa_splits gives it for either element type)
+  // b200_fmha_fwd_f16_gqa_splits gives it for either element type); a paged call is the seqlens call on the padded Nk
   const int splits = num_splits == 0 ? auto_splits(B, Hkv, G, Nq, Nk, D) : num_splits;
   const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
   return fmha_run<T, KV>(q, k, v, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
-                         static_cast<cudaStream_t>(stream), &lens, nullptr, 0, v_scale);
-}
-
-template <typename T, typename KV = T>
-int fmha_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
-                            const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv,
-                            int Nq, int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
-                            int num_splits, float scale, void* stream, float k_scale = 1.f, float v_scale = 1.f) {
-  if (!q || !k_cache || !v_cache || !o || !block_table)
-    return fail(B200_EINVAL, "fmha_paged: null pointer (q, k_cache, v_cache, o and block_table are required)");
-  if (B <= 0 || H <= 0 || D <= 0) return fail(B200_EINVAL, "fmha_paged: bad shape B=%d H=%d D=%d", B, H, D);
-  if (Nq <= 0) return fail(B200_EINVAL, "fmha_paged: bad length Nq=%d (must be >= 1)", Nq);
-  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_paged: causal must be 0 or 1, got %d", causal);
-  if (Hkv <= 0 || H % Hkv != 0)
-    return fail(B200_EINVAL, "fmha_paged: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
-  if (num_splits < 0 || num_splits > kMaxSplits)
-    return fail(B200_EINVAL, "fmha_paged: num_splits=%d must be in 0 .. %d", num_splits, kMaxSplits);
-  if (static_cast<long long>(B) * Hkv > 65535)
-    return fail(B200_EINVAL, "fmha_paged: B*Hkv = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
-  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
-    return fail(B200_EINVAL,
-                "fmha_paged: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)");
-  if (static_cast<long long>(H / Hkv) * Nq > 0x7FFFFFFFll)
-    return fail(B200_EINVAL, "fmha_paged: (H/Hkv)*Nq = %lld query rows per K/V head exceed 2^31 - 1",
-                static_cast<long long>(H / Hkv) * Nq);
-  if ((reinterpret_cast<uintptr_t>(seqlens_q) & 3u) != 0)
-    return fail(B200_EINVAL, "fmha_paged: seqlens_q must be 4-byte aligned (int32)");
-  if ((reinterpret_cast<uintptr_t>(seqlens_k) & 3u) != 0)
-    return fail(B200_EINVAL, "fmha_paged: seqlens_k must be 4-byte aligned (int32)");
-  if ((reinterpret_cast<uintptr_t>(block_table) & 3u) != 0)
-    return fail(B200_EINVAL, "fmha_paged: block_table must be 4-byte aligned (int32)");
-  if (num_pages < 1) return fail(B200_EINVAL, "fmha_paged: num_pages=%d must be >= 1", num_pages);
-  if (max_pages_per_seq < 1)
-    return fail(B200_EINVAL, "fmha_paged: max_pages_per_seq=%d must be >= 1", max_pages_per_seq);
-  if (page_size < 16 || (page_size & (page_size - 1)) != 0)
-    return fail(B200_EINVAL, "fmha_paged: page_size=%d must be a power of two >= 16", page_size);
-  if (static_cast<long long>(num_pages) * page_size > 0x7FFFFFFFll)
-    return fail(B200_EINVAL, "fmha_paged: num_pages*page_size = %lld pool rows exceed 2^31 - 1",
-                static_cast<long long>(num_pages) * page_size);
-  if (static_cast<long long>(max_pages_per_seq) * page_size > 0x7FFFFFFFll)
-    return fail(B200_EINVAL, "fmha_paged: max_pages_per_seq*page_size = %lld keys per sequence exceed 2^31 - 1",
-                static_cast<long long>(max_pages_per_seq) * page_size);
-  if (D % 8 != 0) return fail(B200_ENOTSUP, "fmha_paged: headdim not support! (D=%d must be a multiple of 8)", D);
-  if (D > 1024) return fail(B200_ENOTSUP, "fmha_paged: headdim not support! (D=%d > 1024)", D);
-  if constexpr (!std::is_same_v<KV, T>) {
-    if (int rc = fp8kv_scales("fmha_paged", D, k_scale, v_scale, &scale)) return rc;
-  }
-  if (!(scale > 0.f)) scale = 1.0f / sqrtf(static_cast<float>(D));
-  const int G = H / Hkv, Nk = max_pages_per_seq * page_size;
-  // everything but the K/V addressing is the seqlens call on the padded Nk, the split count included
-  const int splits = num_splits == 0 ? auto_splits(B, Hkv, G, Nq, Nk, D) : num_splits;
-  const attn::Lens lens{seqlens_q, seqlens_k, Hkv};
-  const attn::Pages pages{block_table, page_size, max_pages_per_seq};
-  return fmha_run<T, KV>(q, k_cache, v_cache, o, lse, 0.f, B, Hkv, G, Nq, Nk, D, false, causal == 1, scale, splits,
-                         static_cast<cudaStream_t>(stream), &lens, &pages, num_pages, v_scale);
+                         static_cast<cudaStream_t>(stream), &lens, pages, num_pages, v_scale);
 }
 
 // b200_fmha_fwd_{f16,bf16}_varlen (table == nullptr: cu_k is cu_seqlens_k, K / V [total_k, Hkv, D]) and _varlen_paged
@@ -507,38 +499,21 @@ int fmha_varlen(const char* who, const void* q, const void* k, const void* v, vo
   if (max_q <= 0) return fail(B200_EINVAL, "%s: max_seqlen_q=%d must be >= 1", who, max_q);
   if (!paged && max_k <= 0) return fail(B200_EINVAL, "%s: max_seqlen_k=%d must be >= 1", who, max_k);
   if (causal != 0 && causal != 1) return fail(B200_EINVAL, "%s: causal must be 0 or 1, got %d", who, causal);
-  if (Hkv <= 0 || H % Hkv != 0) return fail(B200_EINVAL, "%s: Hkv=%d must be >= 1 and divide H=%d", who, Hkv, H);
-  if (static_cast<long long>(B) * Hkv > 65535)
-    return fail(B200_EINVAL, "%s: B*Hkv = %lld exceeds the grid limit 65535", who, static_cast<long long>(B) * Hkv);
-  if ((reinterpret_cast<uintptr_t>(cu_q) & 3u) != 0)
-    return fail(B200_EINVAL, "%s: cu_seqlens_q must be 4-byte aligned (int32)", who);
-  if ((reinterpret_cast<uintptr_t>(cu_k) & 3u) != 0)
-    return fail(B200_EINVAL, paged ? "%s: seqused_k must be 4-byte aligned (int32)"
-                                   : "%s: cu_seqlens_k must be 4-byte aligned (int32)", who);
+  if (int rc = check_hkv(who, H, Hkv)) return rc;
+  if (int rc = check_grid_heads(who, "B*Hkv", B, Hkv)) return rc;
+  if (int rc = check_int32(who, cu_q, "cu_seqlens_q")) return rc;
+  if (int rc = check_int32(who, cu_k, paged ? "seqused_k" : "cu_seqlens_k")) return rc;
   if (paged) {
-    if ((reinterpret_cast<uintptr_t>(table) & 3u) != 0)
-      return fail(B200_EINVAL, "%s: block_table must be 4-byte aligned (int32)", who);
-    if (num_pages < 1) return fail(B200_EINVAL, "%s: num_pages=%d must be >= 1", who, num_pages);
-    if (max_pages < 1) return fail(B200_EINVAL, "%s: max_pages_per_seq=%d must be >= 1", who, max_pages);
-    if (page_size < 16 || (page_size & (page_size - 1)) != 0)
-      return fail(B200_EINVAL, "%s: page_size=%d must be a power of two >= 16", who, page_size);
-    if (static_cast<long long>(num_pages) * page_size > 0x7FFFFFFFll)
-      return fail(B200_EINVAL, "%s: num_pages*page_size = %lld pool rows exceed 2^31 - 1", who,
-                  static_cast<long long>(num_pages) * page_size);
-    if (static_cast<long long>(max_pages) * page_size > 0x7FFFFFFFll)
-      return fail(B200_EINVAL, "%s: max_pages_per_seq*page_size = %lld keys per sequence exceed 2^31 - 1", who,
-                  static_cast<long long>(max_pages) * page_size);
+    if (int rc = check_int32(who, table, "block_table")) return rc;
+    if (int rc = check_pool(who, num_pages, page_size, max_pages)) return rc;
   }
-  if (D % 8 != 0) return fail(B200_ENOTSUP, "%s: headdim not support! (D=%d must be a multiple of 8)", who, D);
-  if (D > 1024) return fail(B200_ENOTSUP, "%s: headdim not support! (D=%d > 1024)", who, D);
+  if (int rc = check_head_dim(who, D)) return rc;
   // the bytes of q / o must be addressable in int64 (k / v: rows < 2^31 times Hkv <= 65535 times D <= 1024 are)
   if (static_cast<long long>(total_q) * H > 0x3FFFFFFFFFFFFFFFll / D)
     return fail(B200_EINVAL, "%s: total_q*H*D = %d*%d*%d elements overflow", who, total_q, H, D);
   const long long kv_rows = paged ? static_cast<long long>(num_pages) * page_size : total_k;
   const int G = H / Hkv;
-  if (static_cast<long long>(G) * max_q > 0x7FFFFFFFll)
-    return fail(B200_EINVAL, "%s: (H/Hkv)*max_seqlen_q = %lld query rows per K/V head exceed 2^31 - 1", who,
-                static_cast<long long>(G) * max_q);
+  if (int rc = check_rows(who, G, max_q, "max_seqlen_q")) return rc;
   const Family f = family(D);
   const int tph = (max_q + 64 * f.wgs - 1) / (64 * f.wgs), slabs = (D + f.ds - 1) / f.ds;
   if (static_cast<long long>(G) * tph * slabs > 0x7FFFFFFFll)
@@ -548,23 +523,9 @@ int fmha_varlen(const char* who, const void* q, const void* k, const void* v, vo
 
   const int nk_pad = paged ? max_pages * page_size : max_k;   // the clamp of every sequence's keys
   attn::Params p;
-  p.Nq = G * max_q;
-  p.qpos = max_q;
-  p.Nk = nk_pad;
-  p.D = D;
-  p.nq = (D + 63) / 64;
-  p.num_kv = (nk_pad + f.bn - 1) / f.bn;
-  p.diag = nk_pad - max_q;
-  p.slabs = slabs;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  p.lse = lse;
-  p.rms_g = 0.f;
-  p.o_ptr = static_cast<__half*>(o);
-  p.ws_o = nullptr;
-  p.ws_lse = nullptr;
-  p.tph = tph;
-  const int smem = ring_smem(f, p.nq, false, 0, &p.ring);
+  const int smem = attn_params(&p, G, max_q, nk_pad, D, scale, lse, 0.f, o, false, 0);
   if (smem == 0) return fail(B200_ENOTSUP, "%s: headdim not support! (D=%d)", who, D);
+  p.tph = tph;
 
   constexpr bool bf16 = std::is_same_v<T, __nv_bfloat16>;
   const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
@@ -576,14 +537,8 @@ int fmha_varlen(const char* who, const void* q, const void* k, const void* v, vo
   if ((rc = rows_map(&tv, v, D, Hkv, static_cast<uint64_t>(kv_rows), box, 2, dt))) return rc;
   const attn::Varlen vl{cu_q, cu_k, total_q, H, Hkv};
   const attn::Pages pages{table, page_size, max_pages};
-  const attn::Pages* pg = paged ? &pages : nullptr;
-  const int bh = B * Hkv, qtiles = G * tph;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (f.ds == 64)
-    return attn::launch_attn_varlen<T, 64, 128, 2>(tq, tk, tv, p, qtiles, bh, smem, causal == 1, vl, pg, st);
-  if (f.ds == 128)
-    return attn::launch_attn_varlen<T, 128, 64, 2>(tq, tk, tv, p, qtiles, bh, smem, causal == 1, vl, pg, st);
-  return attn::launch_attn_varlen<T, 256, 64, 1>(tq, tk, tv, p, qtiles, bh, smem, causal == 1, vl, pg, st);
+  const attn::Launch l{tq, tk, tv, p, G * tph, B * Hkv, 1, smem, static_cast<cudaStream_t>(stream)};
+  return attn::launch_attn_varlen<T>(l, causal == 1, vl, paged ? &pages : nullptr);
 }
 
 }  // namespace
@@ -603,31 +558,20 @@ int b200_fmha_fwd_f16_lse(const void* q, const void* k, const void* v, void* o, 
 
 int b200_fmha_fwd_f16_kv(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int Nq,
                          int Nk, int D, int v_transposed, int causal, float scale, void* stream) {
-  if (Nq <= 0 || Nk <= 0) return fail(B200_EINVAL, "fmha_kv: bad lengths Nq=%d Nk=%d (both must be >= 1)", Nq, Nk);
-  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_kv: causal must be 0 or 1, got %d", causal);
-  if (v_transposed && (Nk % 8) != 0)
-    return fail(B200_EINVAL, "fmha_kv: Nk (%d) must be a multiple of 8 for transposed V", Nk);
+  if (int rc = check_kv("fmha_kv", Nq, Nk, v_transposed, causal)) return rc;
   return fmha_impl(q, k, v, o, lse, B, H, Nq, Nk, D, v_transposed, causal == 1, scale, stream);
 }
 
 int b200_fmha_fwd_f16_gqa(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int Hkv,
                           int Nq, int Nk, int D, int v_transposed, int causal, int num_splits, float scale,
                           void* stream) {
-  if (Nq <= 0 || Nk <= 0) return fail(B200_EINVAL, "fmha_gqa: bad lengths Nq=%d Nk=%d (both must be >= 1)", Nq, Nk);
-  if (causal != 0 && causal != 1) return fail(B200_EINVAL, "fmha_gqa: causal must be 0 or 1, got %d", causal);
-  if (v_transposed && (Nk % 8) != 0)
-    return fail(B200_EINVAL, "fmha_gqa: Nk (%d) must be a multiple of 8 for transposed V", Nk);
-  if (Hkv <= 0 || H % Hkv != 0)
-    return fail(B200_EINVAL, "fmha_gqa: Hkv=%d must be >= 1 and divide H=%d", Hkv, H);
-  if (num_splits < 0 || num_splits > kMaxSplits)
-    return fail(B200_EINVAL, "fmha_gqa: num_splits=%d must be in 0 .. %d", num_splits, kMaxSplits);
-  if (static_cast<long long>(B) * Hkv > 65535)
-    return fail(B200_EINVAL, "fmha_gqa: B*Hkv = %lld exceeds the grid limit 65535", static_cast<long long>(B) * Hkv);
-  if (num_splits != 1 && (reinterpret_cast<uintptr_t>(o) & 15u) != 0)
-    return fail(B200_EINVAL, "fmha_gqa: o must be 16-byte aligned when num_splits != 1 (the combine stores 16 bytes)");
-  if (static_cast<long long>(H / Hkv) * Nq > 0x7FFFFFFFll)
-    return fail(B200_EINVAL, "fmha_gqa: (H/Hkv)*Nq = %lld query rows per K/V head exceed 2^31 - 1",
-                static_cast<long long>(H / Hkv) * Nq);
+  const char* who = "fmha_gqa";
+  if (int rc = check_kv(who, Nq, Nk, v_transposed, causal)) return rc;
+  if (int rc = check_hkv(who, H, Hkv)) return rc;
+  if (int rc = check_splits(who, num_splits)) return rc;
+  if (int rc = check_grid_heads(who, "B*Hkv", B, Hkv)) return rc;
+  if (int rc = check_split_out(who, num_splits, o)) return rc;
+  if (int rc = check_rows(who, H / Hkv, Nq, "Nq")) return rc;
   return fmha_impl(q, k, v, o, lse, B, H, Nq, Nk, D, v_transposed, causal == 1, scale, stream, 0.f, H / Hkv,
                    num_splits);
 }
@@ -643,56 +587,58 @@ int b200_fmha_fwd_f16_gqa_splits(int B, int H, int Hkv, int Nq, int Nk, int D) {
 int b200_fmha_fwd_f16_seqlens(const void* q, const void* k, const void* v, void* o, float* lse, const int* seqlens_q,
                               const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk, int D, int causal,
                               int num_splits, float scale, void* stream) {
-  return fmha_seqlens<__half>(q, k, v, o, lse, seqlens_q, seqlens_k, B, H, Hkv, Nq, Nk, D, causal, num_splits, scale,
-                              stream);
+  return fmha_lens<__half>(q, k, v, o, lse, seqlens_q, seqlens_k, nullptr, 0, B, H, Hkv, Nq, Nk, D, causal, num_splits,
+                           scale, stream);
 }
 
 int b200_fmha_fwd_f16_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
                             const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv,
                             int Nq, int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
                             int num_splits, float scale, void* stream) {
-  return fmha_paged<__half>(q, k_cache, v_cache, o, lse, block_table, seqlens_q, seqlens_k, B, H, Hkv, Nq, num_pages,
-                            page_size, max_pages_per_seq, D, causal, num_splits, scale, stream);
+  const attn::Pages pages{block_table, page_size, max_pages_per_seq};
+  return fmha_lens<__half>(q, k_cache, v_cache, o, lse, seqlens_q, seqlens_k, &pages, num_pages, B, H, Hkv, Nq, 0, D,
+                           causal, num_splits, scale, stream);
 }
 
 int b200_fmha_fwd_bf16_seqlens(const void* q, const void* k, const void* v, void* o, float* lse, const int* seqlens_q,
                                const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk, int D, int causal,
                                int num_splits, float scale, void* stream) {
-  return fmha_seqlens<__nv_bfloat16>(q, k, v, o, lse, seqlens_q, seqlens_k, B, H, Hkv, Nq, Nk, D, causal, num_splits,
-                                     scale, stream);
+  return fmha_lens<__nv_bfloat16>(q, k, v, o, lse, seqlens_q, seqlens_k, nullptr, 0, B, H, Hkv, Nq, Nk, D, causal,
+                                  num_splits, scale, stream);
 }
 
 int b200_fmha_fwd_bf16_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
                              const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv,
                              int Nq, int num_pages, int page_size, int max_pages_per_seq, int D, int causal,
                              int num_splits, float scale, void* stream) {
-  return fmha_paged<__nv_bfloat16>(q, k_cache, v_cache, o, lse, block_table, seqlens_q, seqlens_k, B, H, Hkv, Nq,
-                                   num_pages, page_size, max_pages_per_seq, D, causal, num_splits, scale, stream);
+  const attn::Pages pages{block_table, page_size, max_pages_per_seq};
+  return fmha_lens<__nv_bfloat16>(q, k_cache, v_cache, o, lse, seqlens_q, seqlens_k, &pages, num_pages, B, H, Hkv, Nq,
+                                  0, D, causal, num_splits, scale, stream);
 }
 
 int b200_fmha_fwd_f16_fp8kv_seqlens(const void* q, const void* k, const void* v, void* o, float* lse,
                                     const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk,
                                     int D, int causal, int num_splits, float scale, float k_scale, float v_scale,
                                     void* stream) {
-  return fmha_seqlens<__half, __nv_fp8_e4m3>(q, k, v, o, lse, seqlens_q, seqlens_k, B, H, Hkv, Nq, Nk, D, causal,
-                                             num_splits, scale, stream, k_scale, v_scale);
+  return fmha_lens<__half, __nv_fp8_e4m3>(q, k, v, o, lse, seqlens_q, seqlens_k, nullptr, 0, B, H, Hkv, Nq, Nk, D,
+                                          causal, num_splits, scale, stream, k_scale, v_scale);
 }
 
 int b200_fmha_fwd_bf16_fp8kv_seqlens(const void* q, const void* k, const void* v, void* o, float* lse,
                                      const int* seqlens_q, const int* seqlens_k, int B, int H, int Hkv, int Nq, int Nk,
                                      int D, int causal, int num_splits, float scale, float k_scale, float v_scale,
                                      void* stream) {
-  return fmha_seqlens<__nv_bfloat16, __nv_fp8_e4m3>(q, k, v, o, lse, seqlens_q, seqlens_k, B, H, Hkv, Nq, Nk, D, causal,
-                                                    num_splits, scale, stream, k_scale, v_scale);
+  return fmha_lens<__nv_bfloat16, __nv_fp8_e4m3>(q, k, v, o, lse, seqlens_q, seqlens_k, nullptr, 0, B, H, Hkv, Nq, Nk,
+                                                 D, causal, num_splits, scale, stream, k_scale, v_scale);
 }
 
 int b200_fmha_fwd_f16_fp8kv_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
                                   const int* block_table, const int* seqlens_q, const int* seqlens_k, int B, int H,
                                   int Hkv, int Nq, int num_pages, int page_size, int max_pages_per_seq, int D,
                                   int causal, int num_splits, float scale, float k_scale, float v_scale, void* stream) {
-  return fmha_paged<__half, __nv_fp8_e4m3>(q, k_cache, v_cache, o, lse, block_table, seqlens_q, seqlens_k, B, H, Hkv,
-                                           Nq, num_pages, page_size, max_pages_per_seq, D, causal, num_splits, scale,
-                                           stream, k_scale, v_scale);
+  const attn::Pages pages{block_table, page_size, max_pages_per_seq};
+  return fmha_lens<__half, __nv_fp8_e4m3>(q, k_cache, v_cache, o, lse, seqlens_q, seqlens_k, &pages, num_pages, B, H,
+                                          Hkv, Nq, 0, D, causal, num_splits, scale, stream, k_scale, v_scale);
 }
 
 int b200_fmha_fwd_bf16_fp8kv_paged(const void* q, const void* k_cache, const void* v_cache, void* o, float* lse,
@@ -700,9 +646,10 @@ int b200_fmha_fwd_bf16_fp8kv_paged(const void* q, const void* k_cache, const voi
                                    int Hkv, int Nq, int num_pages, int page_size, int max_pages_per_seq, int D,
                                    int causal, int num_splits, float scale, float k_scale, float v_scale,
                                    void* stream) {
-  return fmha_paged<__nv_bfloat16, __nv_fp8_e4m3>(q, k_cache, v_cache, o, lse, block_table, seqlens_q, seqlens_k, B, H,
-                                                  Hkv, Nq, num_pages, page_size, max_pages_per_seq, D, causal,
-                                                  num_splits, scale, stream, k_scale, v_scale);
+  const attn::Pages pages{block_table, page_size, max_pages_per_seq};
+  return fmha_lens<__nv_bfloat16, __nv_fp8_e4m3>(q, k_cache, v_cache, o, lse, seqlens_q, seqlens_k, &pages, num_pages,
+                                                 B, H, Hkv, Nq, 0, D, causal, num_splits, scale, stream, k_scale,
+                                                 v_scale);
 }
 
 int b200_fmha_fwd_f16_varlen(const void* q, const void* k, const void* v, void* o, float* lse, const int* cu_seqlens_q,

@@ -6,39 +6,17 @@
 namespace b200 {
 namespace attn {
 
-template <typename T, int kDS, int kBN, int kWG>
-int launch_attn_fp8kv(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const Params& p, int qtiles,
-                      int BH, int smem, bool causal, int splits, const Lens& lens, const Pages* pages, float v_scale,
-                      cudaStream_t stream) {
-  if (pages != nullptr) {
-    auto kern = splits > 1 ? (causal ? attn_fwd_fp8kv_paged_kernel<kDS, kBN, kWG, true, true, T>
-                                     : attn_fwd_fp8kv_paged_kernel<kDS, kBN, kWG, false, true, T>)
-                           : (causal ? attn_fwd_fp8kv_paged_kernel<kDS, kBN, kWG, true, false, T>
-                                     : attn_fwd_fp8kv_paged_kernel<kDS, kBN, kWG, false, false, T>);
-    static int attr_smem[4][64] = {};
-    return launch_kernel(kern, attr_smem[2 * (splits > 1) + causal], p, qtiles, BH, splits, threads<kWG>(), smem,
-                         stream, tq, tk, tv, p, lens, *pages, v_scale);
-  }
-  auto kern = splits > 1 ? (causal ? attn_fwd_fp8kv_seqlens_kernel<kDS, kBN, kWG, true, true, T>
-                                   : attn_fwd_fp8kv_seqlens_kernel<kDS, kBN, kWG, false, true, T>)
-                         : (causal ? attn_fwd_fp8kv_seqlens_kernel<kDS, kBN, kWG, true, false, T>
-                                   : attn_fwd_fp8kv_seqlens_kernel<kDS, kBN, kWG, false, false, T>);
-  static int attr_smem[4][64] = {};
-  return launch_kernel(kern, attr_smem[2 * (splits > 1) + causal], p, qtiles, BH, splits, threads<kWG>(), smem, stream,
-                       tq, tk, tv, p, lens, v_scale);
+template <typename T>
+int launch_attn_fp8kv(const Launch& l, bool causal, const Lens& lens, const Pages* pages, float v_scale) {
+  return with_family(l.p.D, [&](auto f) {
+    using F = decltype(f);
+    return with_flags(causal, l.splits > 1, [&](auto c, auto s) {
+      if (pages != nullptr)
+        return launch<attn_fwd_fp8kv_paged_kernel<F::kDS, F::kBN, F::kWG, c, s, T>, F::kWG>(l, lens, *pages, v_scale);
+      return launch<attn_fwd_fp8kv_seqlens_kernel<F::kDS, F::kBN, F::kWG, c, s, T>, F::kWG>(l, lens, v_scale);
+    });
+  });
 }
-
-// the families of attn_capi.cu's family(D): D <= 64, 64 < D <= 128, D > 128
-#define B200_ATTN_FP8KV_INSTANTIATE(T)                                                                                 \
-  template int launch_attn_fp8kv<T, 64, 128, 2>(const CUtensorMap&, const CUtensorMap&, const CUtensorMap&,           \
-                                                const Params&, int, int, int, bool, int, const Lens&, const Pages*,    \
-                                                float, cudaStream_t);                                                  \
-  template int launch_attn_fp8kv<T, 128, 64, 2>(const CUtensorMap&, const CUtensorMap&, const CUtensorMap&,           \
-                                                const Params&, int, int, int, bool, int, const Lens&, const Pages*,    \
-                                                float, cudaStream_t);                                                  \
-  template int launch_attn_fp8kv<T, 256, 64, 1>(const CUtensorMap&, const CUtensorMap&, const CUtensorMap&,           \
-                                                const Params&, int, int, int, bool, int, const Lens&, const Pages*,    \
-                                                float, cudaStream_t);
 
 }  // namespace attn
 }  // namespace b200

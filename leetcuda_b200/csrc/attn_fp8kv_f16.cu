@@ -5,7 +5,7 @@
 namespace b200 {
 namespace attn {
 
-B200_ATTN_FP8KV_INSTANTIATE(__half)
+template int launch_attn_fp8kv<__half>(const Launch&, bool, const Lens&, const Pages*, float);
 
 }  // namespace attn
 }  // namespace b200

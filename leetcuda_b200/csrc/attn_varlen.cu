@@ -5,30 +5,18 @@
 namespace b200 {
 namespace attn {
 
-template <typename T, int kDS, int kBN, int kWG>
-int launch_attn_varlen(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const Params& p, int qtiles,
-                       int BH, int smem, bool causal, const Varlen& vl, const Pages* pages, cudaStream_t stream) {
-  auto kern = pages != nullptr ? (causal ? attn_varlen_kernel<kDS, kBN, kWG, true, true, T>
-                                         : attn_varlen_kernel<kDS, kBN, kWG, false, true, T>)
-                               : (causal ? attn_varlen_kernel<kDS, kBN, kWG, true, false, T>
-                                         : attn_varlen_kernel<kDS, kBN, kWG, false, false, T>);
-  static int attr_smem[4][64] = {};
-  return launch_kernel(kern, attr_smem[2 * (pages != nullptr) + causal], p, qtiles, BH, 1, threads<kWG>(), smem, stream,
-                       tq, tk, tv, p, vl, pages != nullptr ? *pages : Pages{});
+template <typename T>
+int launch_attn_varlen(const Launch& l, bool causal, const Varlen& vl, const Pages* pages) {
+  return with_family(l.p.D, [&](auto f) {
+    using F = decltype(f);
+    return with_flags(causal, pages != nullptr, [&](auto c, auto paged) {
+      return launch<attn_varlen_kernel<F::kDS, F::kBN, F::kWG, c, paged, T>, F::kWG>(l, vl, paged ? *pages : Pages{});
+    });
+  });
 }
 
-// the families of attn_capi.cu's family(D): D <= 64, 64 < D <= 128, D > 128
-#define B200_VARLEN_FAMILY(T, DS, BN, WG)                                                                             \
-  template int launch_attn_varlen<T, DS, BN, WG>(const CUtensorMap&, const CUtensorMap&, const CUtensorMap&,          \
-                                                 const Params&, int, int, int, bool, const Varlen&, const Pages*,     \
-                                                 cudaStream_t);
-B200_VARLEN_FAMILY(__half, 64, 128, 2)
-B200_VARLEN_FAMILY(__half, 128, 64, 2)
-B200_VARLEN_FAMILY(__half, 256, 64, 1)
-B200_VARLEN_FAMILY(__nv_bfloat16, 64, 128, 2)
-B200_VARLEN_FAMILY(__nv_bfloat16, 128, 64, 2)
-B200_VARLEN_FAMILY(__nv_bfloat16, 256, 64, 1)
-#undef B200_VARLEN_FAMILY
+template int launch_attn_varlen<__half>(const Launch&, bool, const Varlen&, const Pages*);
+template int launch_attn_varlen<__nv_bfloat16>(const Launch&, bool, const Varlen&, const Pages*);
 
 }  // namespace attn
 }  // namespace b200

@@ -1,7 +1,7 @@
 // capi_common.cuh — host-side helpers shared by the C-ABI translation units:
 // error text, launch counter, driver entry point for cuTensorMapEncodeTiled
 // (resolved at run time so the library loads on a machine without libcuda),
-// and a small cache of encoded tensor maps.
+// a small cache of encoded tensor maps, and the persistent cluster launch of the GEMMs.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -32,6 +32,51 @@ void count_launch(uint64_t n = 1);
   } while (0)
 
 int sm_count();  // SMs of the current device (cached per device)
+
+// Persistent launch of Kern(args...) in clusters of `cs` CTAs (1 or 2) over num_tiles cluster tiles, with `threads`
+// threads and `smem` bytes of dynamic shared memory per CTA.  A cluster of two occupies two SMs of one GPC, so with
+// cs = 2 the grid is as many clusters as fit the GPU at once (cached per device), not #SMs / 2: a GPC with an odd
+// number of SMs then leaves one SM idle instead of running a cluster in a second wave.  who prefixes the error.
+template <auto Kern, typename... Args>
+int launch_persistent(const char* who, int threads, int smem, int num_tiles, int cs, cudaStream_t stream,
+                      const Args&... args) {
+  static bool attr_set[64] = {false};
+  static int max_clusters[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const bool cached = dev >= 0 && dev < 64;
+  if (!cached || !attr_set[dev]) {
+    B200_CUDA_OK(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    if (cached) attr_set[dev] = true;
+  }
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.blockDim = dim3(threads, 1, 1);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attrs[1];
+  attrs[0].id = cudaLaunchAttributeClusterDimension;
+  attrs[0].val.clusterDim.x = static_cast<unsigned>(cs);
+  attrs[0].val.clusterDim.y = 1;
+  attrs[0].val.clusterDim.z = 1;
+  cfg.attrs = attrs;
+  cfg.numAttrs = 1;
+  int slots = sm_count();
+  if (cs > 1) {
+    slots = cached ? max_clusters[dev] : 0;
+    if (slots == 0) {
+      cfg.gridDim = dim3(static_cast<unsigned>(cs), 1, 1);
+      B200_CUDA_OK(cudaOccupancyMaxActiveClusters(&slots, Kern, &cfg));
+      if (slots <= 0) return fail(B200_ECUDA, "%s: no cluster of %d CTAs fits the device", who, cs);
+      if (cached) max_clusters[dev] = slots;
+    }
+  }
+  const int grid = cs * (num_tiles < slots ? num_tiles : slots);
+  cfg.gridDim = dim3(static_cast<unsigned>(grid), 1, 1);
+  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, Kern, args...));
+  count_launch();
+  return 0;
+}
 
 // Do the byte ranges [a, a + na) and [b, b + nb) share a byte?
 inline bool overlaps(const void* a, size_t na, const void* b, size_t nb) {

@@ -9,49 +9,12 @@ using namespace b200;
 using b200::host::fail;
 using b200::host::overlaps;
 
-// Persistent launch in clusters of `cs` CTAs, sized as launch_hgemm sizes it (hgemm_capi.cu): with cs = 2 the grid is
-// as many clusters as fit the GPU at once (cached per device), so no cluster waits for a second wave.
+// Persistent launch in clusters of `cs` CTAs, as launch_hgemm (hgemm_capi.cu)
 template <typename OutT, bool kBlockScale>
 int launch_gemm_e4m3(const CUtensorMap& ta, const CUtensorMap& tb, const gemm_fp8::Params& p, int cs,
                      cudaStream_t stream) {
-  using C_ = gemm_fp8::C_;
-  auto kern = gemm_fp8::gemm_e4m3_kernel<OutT, kBlockScale>;
-  static bool attr_set[64] = {false};
-  static int max_clusters[64] = {0};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  const bool cached = dev >= 0 && dev < 64;
-  if (!cached || !attr_set[dev]) {
-    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES));
-    if (cached) attr_set[dev] = true;
-  }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.blockDim = dim3(gemm_fp8::kThreads, 1, 1);
-  cfg.dynamicSmemBytes = C_::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeClusterDimension;
-  attrs[0].val.clusterDim.x = static_cast<unsigned>(cs);
-  attrs[0].val.clusterDim.y = 1;
-  attrs[0].val.clusterDim.z = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = 1;
-  int slots = host::sm_count();
-  if (cs > 1) {
-    slots = cached ? max_clusters[dev] : 0;
-    if (slots == 0) {
-      cfg.gridDim = dim3(static_cast<unsigned>(cs), 1, 1);
-      B200_CUDA_OK(cudaOccupancyMaxActiveClusters(&slots, kern, &cfg));
-      if (slots <= 0) return fail(B200_ECUDA, "gemm_e4m3: no cluster of %d CTAs fits the device", cs);
-      if (cached) max_clusters[dev] = slots;
-    }
-  }
-  const int grid = cs * (p.g.num_tiles < slots ? p.g.num_tiles : slots);
-  cfg.gridDim = dim3(static_cast<unsigned>(grid), 1, 1);
-  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, ta, tb, p));
-  host::count_launch();
-  return 0;
+  return host::launch_persistent<gemm_fp8::gemm_e4m3_kernel<OutT, kBlockScale>>(
+      "gemm_e4m3", gemm_fp8::kThreads, gemm_fp8::C_::SMEM_BYTES, p.g.num_tiles, cs, stream, ta, tb, p);
 }
 
 }  // namespace

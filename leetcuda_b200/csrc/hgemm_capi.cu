@@ -10,49 +10,11 @@ namespace {
 using namespace b200;
 using b200::host::fail;
 
-// Persistent launch in clusters of `cs` CTAs (1 or 2; p.num_tiles counts cluster tiles).  A cluster of two occupies two
-// SMs of one GPC, so with cs = 2 the grid is as many clusters as fit the GPU at once (cached per device), not #SMs / 2:
-// a GPC with an odd number of SMs then leaves one SM idle instead of running a cluster in a second wave.
+// Persistent launch in clusters of `cs` CTAs (1 or 2; p.num_tiles counts cluster tiles)
 template <int kBN, bool kBMn, bool kTf32, bool kAcc16>
 int launch_hgemm(const CUtensorMap& ta, const CUtensorMap& tb, const hgemm::Params& p, int cs, cudaStream_t stream) {
-  using C_ = hgemm::Cfg<kBN>;
-  auto kern = hgemm::hgemm_wgmma_kernel<kBN, kBMn, kTf32, kAcc16>;
-  static bool attr_set[64] = {false};
-  static int max_clusters[64] = {0};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  const bool cached = dev >= 0 && dev < 64;
-  if (!cached || !attr_set[dev]) {
-    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES));
-    if (cached) attr_set[dev] = true;
-  }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.blockDim = dim3(hgemm::kThreads, 1, 1);
-  cfg.dynamicSmemBytes = C_::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeClusterDimension;
-  attrs[0].val.clusterDim.x = static_cast<unsigned>(cs);
-  attrs[0].val.clusterDim.y = 1;
-  attrs[0].val.clusterDim.z = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = 1;
-  int slots = host::sm_count();
-  if (cs > 1) {
-    slots = cached ? max_clusters[dev] : 0;
-    if (slots == 0) {
-      cfg.gridDim = dim3(static_cast<unsigned>(cs), 1, 1);
-      B200_CUDA_OK(cudaOccupancyMaxActiveClusters(&slots, kern, &cfg));
-      if (slots <= 0) return fail(B200_ECUDA, "hgemm: no cluster of %d CTAs fits the device", cs);
-      if (cached) max_clusters[dev] = slots;
-    }
-  }
-  const int grid = cs * (p.num_tiles < slots ? p.num_tiles : slots);
-  cfg.gridDim = dim3(static_cast<unsigned>(grid), 1, 1);
-  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, ta, tb, p));
-  host::count_launch();
-  return 0;
+  return host::launch_persistent<hgemm::hgemm_wgmma_kernel<kBN, kBMn, kTf32, kAcc16>>(
+      "hgemm", hgemm::kThreads, hgemm::Cfg<kBN>::SMEM_BYTES, p.num_tiles, cs, stream, ta, tb, p);
 }
 
 // tf32(v): round to nearest, ties away from zero

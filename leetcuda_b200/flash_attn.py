@@ -198,11 +198,7 @@ def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=
             raise RuntimeError("leetcuda_b200.flash_attn: transposed V is not supported with fp8 K/V "
                                "(v_transposed=True with float8_e4m3fn tensors)")
         scales = (float(k_scale), float(v_scale))
-        if block_table is not None:
-            _fmha_paged(Q, K, V, O, False, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table, fp8,
-                        scales)
-        else:
-            _fmha_seqlens(Q, K, V, O, False, scale, lse, causal, num_splits, seqlens_q, seqlens_k, fp8, scales)
+        _fmha_lens(Q, K, V, O, False, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table, fp8, scales)
         return
     if k_scale != 1.0 or v_scale != 1.0:
         raise RuntimeError(f"leetcuda_b200.flash_attn: k_scale / v_scale apply to fp8 (float8_e4m3fn) K and V only, "
@@ -211,39 +207,50 @@ def fmha_fwd(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0, lse=
     dtype = _element_type(Q, K, V, O)
     if dtype == torch.bfloat16 and v_transposed:
         raise RuntimeError("leetcuda_b200.flash_attn: transposed V is fp16 only (v_transposed=True with bf16 tensors)")
-    if block_table is not None:
-        _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table, dtype)
-        return
-    if seqlens_q is not None or seqlens_k is not None or dtype == torch.bfloat16:
-        _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, dtype)
+    if block_table is not None or seqlens_q is not None or seqlens_k is not None or dtype == torch.bfloat16:
+        _fmha_lens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table, dtype)
         return
     B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, v_transposed, same_length=False, grouped=True)
-    if isinstance(num_splits, bool) or not isinstance(num_splits, int) or not 0 <= num_splits <= _capi.FMHA_MAX_SPLITS:
-        raise RuntimeError(f"leetcuda_b200.flash_attn: num_splits must be an int in 0 .. {_capi.FMHA_MAX_SPLITS}, "
-                           f"got {num_splits!r}")
-    if lse is not None and (lse.dtype != torch.float32 or tuple(lse.shape) != (B, H, Nq)):
-        raise RuntimeError("leetcuda_b200.flash_attn: lse must be a contiguous fp32 CUDA tensor [B,H,Nq]")
+    _check_lengths(Q, B, H, Nq, num_splits, lse, None, None)
     _placement(Q, K, V, O, *(() if lse is None else (lse,)))
     _run(Q, K, V, O, B, H, Nq, Nk, D, v_transposed, scale, lse, causal, Hkv, num_splits)
 
 
-def _fmha_seqlens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k,
-                  dtype=torch.float16, fp8_scales=None) -> None:
+def _fmha_lens(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table,
+               dtype=torch.float16, fp8_scales=None) -> None:
+    """The seqlens call (``b200_fmha_fwd_*_seqlens``), or with ``block_table`` the paged one (``..._paged``)."""
+    paged = block_table is not None
     if v_transposed:
-        raise RuntimeError("leetcuda_b200.flash_attn: seqlens_q / seqlens_k take natural V [B,Hkv,Nk,D] only "
+        raise RuntimeError("leetcuda_b200.flash_attn: block_table takes natural V pools [num_pages,page_size,Hkv,D] "
+                           "only (v_transposed=True is not supported with a block table)" if paged else
+                           "leetcuda_b200.flash_attn: seqlens_q / seqlens_k take natural V [B,Hkv,Nk,D] only "
                            "(v_transposed=True is not supported with lengths)")
-    B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, False, same_length=False, grouped=True, dtype=dtype,
-                                   fp8=fp8_scales is not None)
+    if paged:
+        if fp8_scales is None:
+            _check_dtype(Q, K, V, O, dtype)
+        if Q.dim() != 4 or tuple(O.shape) != tuple(Q.shape):
+            raise RuntimeError("Tensor size mismatch!")
+        B, H, Nq, D = Q.shape
+        num_pages, page_size, Hkv = _check_pool("leetcuda_b200.flash_attn", K, V, D, H, "K", "V")
+    else:
+        B, H, Nq, Nk, D, Hkv = _shapes(Q, K, V, O, False, same_length=False, grouped=True, dtype=dtype,
+                                       fp8=fp8_scales is not None)
     _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k)
+    if paged:
+        _check_block_table("leetcuda_b200.flash_attn", block_table, B, Q, "Q's")
     _placement(Q, K, V, O, *(() if lse is None else (lse,)))
-    args = [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), None if lse is None else lse.data_ptr(),
-            None if seqlens_q is None else seqlens_q.data_ptr(), None if seqlens_k is None else seqlens_k.data_ptr(),
-            B, H, Hkv, Nq, Nk, D, int(bool(causal)), int(num_splits), float(scale)]
+    lens = [None if seqlens_q is None else seqlens_q.data_ptr(), None if seqlens_k is None else seqlens_k.data_ptr()]
+    args = [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), None if lse is None else lse.data_ptr()]
+    if paged:
+        args += [block_table.data_ptr()] + lens + [B, H, Hkv, Nq, num_pages, page_size, block_table.shape[1], D]
+    else:
+        args += lens + [B, H, Hkv, Nq, Nk, D]
+    args += [int(bool(causal)), int(num_splits), float(scale)]
     name = "b200_fmha_fwd_bf16" if dtype == torch.bfloat16 else "b200_fmha_fwd_f16"
     if fp8_scales is not None:
         name += "_fp8kv"
         args += list(fp8_scales)
-    _call_on_device(getattr(_capi.lib(), name + "_seqlens"), args, Q.device.index)
+    _call_on_device(getattr(_capi.lib(), name + ("_paged" if paged else "_seqlens")), args, Q.device.index)
 
 
 def _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k) -> None:
@@ -262,40 +269,23 @@ def _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k) -> None:
                                f"on Q's device")
 
 
-def _fmha_paged(Q, K, V, O, v_transposed, scale, lse, causal, num_splits, seqlens_q, seqlens_k, block_table,
-                dtype=torch.float16, fp8_scales=None) -> None:
-    if v_transposed:
-        raise RuntimeError("leetcuda_b200.flash_attn: block_table takes natural V pools [num_pages,page_size,Hkv,D] "
-                           "only (v_transposed=True is not supported with a block table)")
-    if fp8_scales is None:
-        _check_dtype(Q, K, V, O, dtype)
-    if Q.dim() != 4 or tuple(O.shape) != tuple(Q.shape):
-        raise RuntimeError("Tensor size mismatch!")
-    B, H, Nq, D = Q.shape
+def _check_pool(who, K, V, D, H, k_name, v_name):
+    """(num_pages, page_size, Hkv) of the paged K/V pools K and V [num_pages, page_size, Hkv, D]."""
     if K.dim() != 4 or tuple(K.shape) != tuple(V.shape) or K.shape[3] != D or K.shape[2] < 1 or H % K.shape[2] \
             or K.shape[0] < 1:
-        raise RuntimeError(f"leetcuda_b200.flash_attn: with block_table, K and V must be pools "
+        raise RuntimeError(f"{who}: with block_table, {k_name} and {v_name} must be pools "
                            f"[num_pages, page_size, Hkv, D] of the same shape, with D = {D} and Hkv dividing H = {H}")
     num_pages, page_size, Hkv, _ = K.shape
     if page_size < 16 or page_size & (page_size - 1):
-        raise RuntimeError(f"leetcuda_b200.flash_attn: page_size (K.shape[1]) must be a power of two >= 16, "
-                           f"got {page_size}")
-    _check_lengths(Q, B, H, Nq, num_splits, lse, seqlens_q, seqlens_k)
-    t = block_table
+        raise RuntimeError(f"{who}: page_size ({k_name}.shape[1]) must be a power of two >= 16, got {page_size}")
+    return num_pages, page_size, Hkv
+
+
+def _check_block_table(who, t, B, q, q_name) -> None:
     if not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or t.dim() != 2 or t.shape[0] != B \
-            or t.shape[1] < 1 or not t.is_cuda or not t.is_contiguous() or t.device != Q.device:
-        raise RuntimeError(f"leetcuda_b200.flash_attn: block_table must be an int32 contiguous CUDA tensor "
-                           f"[B, max_pages_per_seq] = [{B}, >= 1] on Q's device")
-    _placement(Q, K, V, O, *(() if lse is None else (lse,)))
-    args = [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), None if lse is None else lse.data_ptr(),
-            t.data_ptr(), None if seqlens_q is None else seqlens_q.data_ptr(),
-            None if seqlens_k is None else seqlens_k.data_ptr(), B, H, Hkv, Nq, num_pages, page_size, t.shape[1], D,
-            int(bool(causal)), int(num_splits), float(scale)]
-    name = "b200_fmha_fwd_bf16" if dtype == torch.bfloat16 else "b200_fmha_fwd_f16"
-    if fp8_scales is not None:
-        name += "_fp8kv"
-        args += list(fp8_scales)
-    _call_on_device(getattr(_capi.lib(), name + "_paged"), args, Q.device.index)
+            or t.shape[1] < 1 or not t.is_cuda or not t.is_contiguous() or t.device != q.device:
+        raise RuntimeError(f"{who}: block_table must be an int32 contiguous CUDA tensor "
+                           f"[B, max_pages_per_seq] = [{B}, >= 1] on {q_name} device")
 
 
 def fmha_varlen_fwd(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q: int, max_seqlen_k: int, *,
@@ -358,13 +348,7 @@ def fmha_varlen_fwd(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q: int, m
     if paged:
         if cu_seqlens_k is not None:
             raise RuntimeError(f"{who}: with block_table, cu_seqlens_k must be None (seqused_k gives the keys)")
-        if k.dim() != 4 or tuple(k.shape) != tuple(v.shape) or k.shape[3] != D or k.shape[2] < 1 or H % k.shape[2] \
-                or k.shape[0] < 1:
-            raise RuntimeError(f"{who}: with block_table, k and v must be pools [num_pages, page_size, Hkv, D] of the "
-                               f"same shape, with D = {D} and Hkv dividing H = {H}")
-        num_pages, page_size, Hkv, _ = k.shape
-        if page_size < 16 or page_size & (page_size - 1):
-            raise RuntimeError(f"{who}: page_size (k.shape[1]) must be a power of two >= 16, got {page_size}")
+        num_pages, page_size, Hkv = _check_pool(who, k, v, D, H, "k", "v")
     else:
         if seqused_k is not None:
             raise RuntimeError(f"{who}: seqused_k needs block_table (packed K/V take their lengths from cu_seqlens_k)")
@@ -379,11 +363,7 @@ def fmha_varlen_fwd(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q: int, m
         raise RuntimeError(f"{who}: cu_seqlens_q must be an int32 contiguous CUDA tensor [B + 1] (B >= 1) on q's device")
     B = cu_seqlens_q.shape[0] - 1
     if paged:
-        t = block_table
-        if not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or t.dim() != 2 or t.shape[0] != B \
-                or t.shape[1] < 1 or not t.is_cuda or not t.is_contiguous() or t.device != q.device:
-            raise RuntimeError(f"{who}: block_table must be an int32 contiguous CUDA tensor "
-                               f"[B, max_pages_per_seq] = [{B}, >= 1] on q's device")
+        _check_block_table(who, block_table, B, q, "q's")
     arrays = [("cu_seqlens_q", cu_seqlens_q, B + 1)]
     arrays += [("seqused_k", seqused_k, B)] if paged else [("cu_seqlens_k", cu_seqlens_k, B + 1)]
     for on_device in (False, True):   # every array's type and shape first, then where it lives
@@ -546,13 +526,7 @@ def _append(who, k, v, k_cache, v_cache, cache_seqlens, block_table, q, q_out, r
         name += "_paged"
     else:
         args = head + mid + [capacity] + tail
-    idx = k.device.index
-    if torch.cuda.current_device() != idx:
-        with torch.cuda.device(idx):
-            rc = getattr(_capi.lib(), name)(*args, _capi.raw_stream(idx))
-    else:
-        rc = getattr(_capi.lib(), name)(*args, _capi.raw_stream(idx))
-    _capi.check(rc, "kvcache_append")
+    _call_on_device(getattr(_capi.lib(), name), args, k.device.index, "kvcache_append", headdim=False)
 
 
 def fmha_fwd_kvcache(q, k_cache, v_cache, o, k, v, cache_seqlens, *, block_table=None, rotary_cos=None,
@@ -598,15 +572,16 @@ def fmha_fwd_kvcache(q, k_cache, v_cache, o, k, v, cache_seqlens, *, block_table
     return new_lens
 
 
-def _call_on_device(fn, args, idx) -> None:
+def _call_on_device(fn, args, idx, label="fmha_fwd", headdim=True) -> None:
+    """fn(*args, stream) on device idx's current stream; headdim: B200_ENOTSUP raises the reference's text."""
     if torch.cuda.current_device() != idx:
         with torch.cuda.device(idx):
             rc = fn(*args, _capi.raw_stream(idx))
     else:
         rc = fn(*args, _capi.raw_stream(idx))
-    if rc == -3:
+    if headdim and rc == -3:  # B200_ENOTSUP: the reference throws exactly this text (flash_attn_mma_split_q.cu:793)
         raise RuntimeError("headdim not support!")
-    _capi.check(rc, "fmha_fwd")
+    _capi.check(rc, label)
 
 
 def _fmha_one_length(Q, K, V, O, v_transposed=False) -> None:
@@ -616,7 +591,6 @@ def _fmha_one_length(Q, K, V, O, v_transposed=False) -> None:
 
 
 def _run(Q, K, V, O, B, H, Nq, Nk, D, v_transposed, scale, lse, causal, Hkv=None, num_splits=1) -> None:
-    idx = Q.device.index
     args = [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr()]
     if (Hkv is not None and Hkv != H) or num_splits != 1:
         fn = _capi.lib().b200_fmha_fwd_f16_gqa
@@ -633,14 +607,7 @@ def _run(Q, K, V, O, B, H, Nq, Nk, D, v_transposed, scale, lse, causal, Hkv=None
         else:
             fn = _capi.lib().b200_fmha_fwd_f16
         args += [B, H, Nq, D, int(v_transposed), float(scale)]
-    if torch.cuda.current_device() != idx:
-        with torch.cuda.device(idx):
-            rc = fn(*args, _capi.raw_stream(idx))
-    else:
-        rc = fn(*args, _capi.raw_stream(idx))
-    if rc == -3:  # B200_ENOTSUP: the reference throws exactly this text (flash_attn_mma_split_q.cu:793)
-        raise RuntimeError("headdim not support!")
-    _capi.check(rc, "fmha_fwd")
+    _call_on_device(fn, args, Q.device.index)
 
 
 def fmha_host(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0) -> None:
@@ -657,11 +624,8 @@ def fmha_host(Q, K, V, O, *, v_transposed: bool = False, scale: float = 0.0) -> 
     if tuple(K.shape) != (B, H, N, D) or tuple(O.shape) != (B, H, N, D) or tuple(V.shape) != want_v:
         raise RuntimeError("Tensor size mismatch!")
     idx = torch.cuda.current_device()
-    rc = _capi.lib().b200_fmha_fwd_f16_host(Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), B, H, N, D,
-                                            int(v_transposed), float(scale), _capi.raw_stream(idx))
-    if rc == -3:
-        raise RuntimeError("headdim not support!")
-    _capi.check(rc, "fmha_host")
+    _call_on_device(_capi.lib().b200_fmha_fwd_f16_host, [Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), B, H,
+                    N, D, int(v_transposed), float(scale)], idx, "fmha_host")
 
 
 def _make(name: str):

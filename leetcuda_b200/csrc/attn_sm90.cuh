@@ -3,7 +3,7 @@
 //   O = softmax(Q K^T * scale) V per (batch, head), fp16 in / out, fp32 scores, statistics and O.
 //
 // One CTA = kWG consumer warpgroups (64 query rows each) + one producer warpgroup (one thread
-// issuing TMA).  Every CTA owns one query tile and one column slab of O (kDS columns); for
+// issuing TMA; a whole warp for paged K/V).  Every CTA owns one query tile and one column slab of O (kDS columns); for
 // D > kDS several CTAs share a query tile and each recomputes S for its slab.
 //
 //   * Q (all of D) stays in shared memory, 64-column chunks of 64 rows, 128B-swizzled;
@@ -251,15 +251,19 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
   const int qtile = kCausal ? gridDim.x / p.slabs - 1 - blockIdx.x / p.slabs : blockIdx.x / p.slabs;
   int q0 = qtile * 64 * kWG;
   int row_end = p.Nq, off = 0;   // kGQA: the rows this CTA stores end before row_end; query position = row - off
-  [[maybe_unused]] int qh = 0, vhk = 0;   // kVarlen: the CTA's query head and K/V head
+  // kSeqlens: the CTA's sequence b and K/V head hk; kVarlen: its query head qh
+  [[maybe_unused]] int b = 0, hk = 0, qh = 0;
+  if constexpr (kSeqlens) {
+    b = blockIdx.y / lens.hkv;
+    hk = blockIdx.y % lens.hkv;
+  }
   if constexpr (kVarlen) {
     // per-head tiles with or without the mask; causal: the longest first across the G heads, as below
     const int x = blockIdx.x / p.slabs, G = gridDim.x / p.slabs / p.tph;
     off = (x % G) * p.qpos;
     q0 = off + (kCausal ? p.tph - 1 - x / G : x / G) * 64 * kWG;
     row_end = off + p.qpos;
-    vhk = blockIdx.y % vl.hkv;
-    qh = vhk * G + x % G;
+    qh = hk * G + x % G;
   } else if constexpr (kCausal && kGQA) {
     if (p.tph > 0) {
       // per-head tiles, the longest first across the G heads of the group, not only within one
@@ -278,7 +282,6 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
   // kVarlen: the sequence's first row of Q / O and (packed K/V) of K / V
   [[maybe_unused]] int qs = 0, ks = 0;
   if constexpr (kVarlen) {
-    const int b = blockIdx.y / vl.hkv;
     qs = __ldg(vl.cu_q + b);
     lq = static_cast<int>(min(max(static_cast<long long>(__ldg(vl.cu_q + b + 1)) - qs, 0ll),
                               static_cast<long long>(p.qpos)));
@@ -295,7 +298,6 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
     // a tile of positions past the sequence: nothing to load, nothing to store (uniform over the CTA, no cluster)
     if (q0 - off >= lq) return;
   } else if constexpr (kSeqlens) {
-    const int b = blockIdx.y / lens.hkv;
     lq = lens.q ? min(max(__ldg(lens.q + b), 0), p.qpos) : p.qpos;
     const int lk = lens.k ? min(max(__ldg(lens.k + b), 0), nk_pad) : nk_pad;
     p.Nk = lk;
@@ -330,115 +332,59 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
 
   if (wg == 0) {
     if constexpr (kWG > 1) reg_dealloc<40>();
-    if constexpr (kPaged) {
-      if (tid < 32) {
-        // lane 0 issues; lane i < nsub holds the pool row of sub-load i of a key block (the top of this file)
-        const int lane = tid, ps = pages.page_size, shift = __ffs(ps) - 1;
-        const int R = min(ps, kBN), nsub = kBN / R;
-        const int hk = blockIdx.y % lens.hkv;
-        const int* table = pages.table + static_cast<size_t>(blockIdx.y / lens.hkv) * pages.max_pages;
-        const int last = ((p.Nk + ps - 1) >> shift) - 1;   // the sequence's last page (p.Nk >= 1 if a block is visited)
-        auto pool_row = [&](int j) {
-          const int t = j * kBN + min(lane, nsub - 1) * R;
-          const unsigned page = static_cast<unsigned>(__ldg(table + min(t >> shift, last)));
-          return static_cast<int>((page << shift) + static_cast<unsigned>(t & (ps - 1)));
-        };
-        if (lane == 0) {
-          prefetch_tmap(&tmap_q);
-          prefetch_tmap(&tmap_k);
-          prefetch_tmap(&tmap_v);
-          mbar_expect_tx(qbar, kWG * p.nq * 8192);
-          for (int w = 0; w < kWG; ++w)
-            for (int c = 0; c < p.nq; ++c) {
-              if constexpr (kVarlen)
-                tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, qh, vrow(qs, q0 - off + 64 * w),
-                            kEvictFirst);
-              else
-                tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, q0 + 64 * w, bh, kEvictFirst);
-            }
-        }
-        int it = 0;
-        int row = kv.x < kv.y ? pool_row(kv.x) : 0;
-        for (int j = kv.x; j < kv.y; ++j) {
-          const int cur = row;
-          if (j + 1 < kv.y) row = pool_row(j + 1);   // one block ahead
-          // the block's K chunks, then its V chunks; the partial block's V onto vbar, as below
-          for (int c = 0; c < p.nq + nvc; ++c, ++it) {
-            const bool isv = c >= p.nq, zeroed = isv && j == vz;
-            const int s = it % p.ring;
-            // kFP8: into the staging slot s, onto staged(s) (rows of R * 64 bytes)
-            const uint32_t bar = kFP8 ? staged(s) : (zeroed ? vbar : full(s));
-            if (lane == 0) {
-              if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
-              if (!zeroed) mbar_expect_tx(bar, kFP8 ? STG : KV_BYTES);
-              else if (c == p.nq) mbar_expect_tx(vbar, nvc * KV_BYTES);
-            }
-            for (int i = 0; i < nsub; ++i) {
-              const int r = __shfl_sync(0xffffffffu, cur, i);
-              if (lane == 0)
-                tma_load_3d(kFP8 ? sstg + s * STG + i * R * 64 : sring + s * SLOT + i * R * 128,
-                            isv ? &tmap_v : &tmap_k, bar, isv ? d0 + 64 * (c - p.nq) : 64 * c, hk, r, kEvictLast);
-            }
-          }
-        }
-      }
-    }
-    if (!kPaged && tid == 0) {
-      prefetch_tmap(&tmap_q);
-      prefetch_tmap(&tmap_k);
-      prefetch_tmap(&tmap_v);
-      mbar_expect_tx(qbar, kWG * p.nq * 8192);
-      for (int w = 0; w < kWG; ++w)
-        for (int c = 0; c < p.nq; ++c) {
-          if constexpr (kVarlen)
-            tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, qh, vrow(qs, q0 - off + 64 * w),
-                        kEvictFirst);
-          else
-            tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, q0 + 64 * w, bh, kEvictFirst);
-        }
-      int it = 0;
-      // kFP8: every K / V chunk goes to the staging slot s, onto staged(s)
-      auto landed = [&](int s) { return kFP8 ? staged(s) : full(s); };
-      auto dst = [&](int s) { return kFP8 ? sstg + s * STG : sring + s * SLOT; };
-      auto next = [&](uint32_t bytes) {
-        const int s = it % p.ring;
-        if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
-        mbar_expect_tx(landed(s), kFP8 ? STG : bytes);
-        ++it;
-        return s;
+    if (kPaged ? tid < 32 : tid == 0) {
+      // lane 0 issues every load.  kPaged: a chunk is nsub sub-loads of R rows, and lane i < nsub holds the pool row of
+      // sub-load i of a key block (the top of this file)
+      const int lane = tid, ps = kPaged ? pages.page_size : kBN, shift = __ffs(ps) - 1;
+      const int R = min(ps, kBN), nsub = kBN / R;
+      const int* table = pages.table + static_cast<size_t>(b) * pages.max_pages;
+      const int last = ((p.Nk + ps - 1) >> shift) - 1;   // the sequence's last page (p.Nk >= 1 if a block is visited)
+      auto pool_row = [&](int j) {
+        const int t = j * kBN + min(lane, nsub - 1) * R;
+        const unsigned page = static_cast<unsigned>(__ldg(table + min(t >> shift, last)));
+        return static_cast<int>((page << shift) + static_cast<unsigned>(t & (ps - 1)));
       };
-      for (int j = kv.x; j < kv.y; ++j) {
-        for (int c = 0; c < p.nq; ++c) {
-          const int s = next(KV_BYTES);
-          if constexpr (kVarlen)
-            tma_load_3d(dst(s), &tmap_k, landed(s), 64 * c, vhk, vrow(ks, j * kBN), kEvictLast);
-          else
-            tma_load_3d(dst(s), &tmap_k, landed(s), 64 * c, j * kBN, bh, kEvictLast);
-        }
-        for (int c = 0; c < nvc; ++c) {
-          if constexpr (kVT) {
-            const int s = next(64 * kDS * 2);
-            tma_load_3d(sring + s * SLOT, &tmap_v, full(s), j * kBN + 64 * c, d0, bh, kEvictLast);
-          } else {
-            if constexpr (kSeqlens) {
-              if (j == vz) {
-                // onto vbar, not the slot's full barrier: warp 1 arrives there once the rows past Lk_b are zero
-                const int s = it % p.ring;
-                if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
-                ++it;
-                if (c == 0) mbar_expect_tx(vbar, nvc * KV_BYTES);
-                if constexpr (kVarlen)
-                  tma_load_3d(sring + s * SLOT, &tmap_v, vbar, d0 + 64 * c, vhk, vrow(ks, j * kBN), kEvictLast);
-                else
-                  tma_load_3d(sring + s * SLOT, &tmap_v, vbar, d0 + 64 * c, j * kBN, bh, kEvictLast);
-                continue;
-              }
-            }
-            const int s = next(KV_BYTES);
+      if (lane == 0) {
+        prefetch_tmap(&tmap_q);
+        prefetch_tmap(&tmap_k);
+        prefetch_tmap(&tmap_v);
+        mbar_expect_tx(qbar, kWG * p.nq * 8192);
+        for (int w = 0; w < kWG; ++w)
+          for (int c = 0; c < p.nq; ++c) {
             if constexpr (kVarlen)
-              tma_load_3d(dst(s), &tmap_v, landed(s), d0 + 64 * c, vhk, vrow(ks, j * kBN), kEvictLast);
+              tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, qh, vrow(qs, q0 - off + 64 * w),
+                          kEvictFirst);
             else
-              tma_load_3d(dst(s), &tmap_v, landed(s), d0 + 64 * c, j * kBN, bh, kEvictLast);
+              tma_load_3d(sq + (w * p.nq + c) * 8192, &tmap_q, qbar, 64 * c, q0 + 64 * w, bh, kEvictFirst);
+          }
+      }
+      int it = 0;
+      int row = kPaged && kv.x < kv.y ? pool_row(kv.x) : 0;
+      for (int j = kv.x; j < kv.y; ++j) {
+        const int cur = row;
+        if (kPaged && j + 1 < kv.y) row = pool_row(j + 1);   // one block ahead
+        // the block's K chunks, then its V chunks, one ring slot each.  The partial block's V (j == vz) lands on vbar,
+        // not on the slots' full barriers: warp 1 arrives there once the rows past Lk_b are zero.
+        for (int c = 0; c < p.nq + nvc; ++c, ++it) {
+          const bool isv = c >= p.nq, zeroed = isv && j == vz;
+          const int s = it % p.ring;
+          // kFP8: into the staging slot s, onto staged(s) (rows of R * 64 bytes)
+          const uint32_t bar = kFP8 ? staged(s) : (zeroed ? vbar : full(s));
+          if (lane == 0) {
+            if (it >= p.ring) mbar_wait(empty(s), ((it / p.ring) - 1) & 1);
+            if (!zeroed) mbar_expect_tx(bar, kFP8 ? STG : (kVT && isv ? 64 * kDS * 2 : KV_BYTES));
+            else if (c == p.nq) mbar_expect_tx(vbar, nvc * KV_BYTES);
+          }
+          const CUtensorMap* map = isv ? &tmap_v : &tmap_k;
+          const int x = isv ? d0 + 64 * (c - p.nq) : 64 * c;
+          for (int i = 0; i < nsub; ++i) {
+            const int r = kPaged ? __shfl_sync(0xffffffffu, cur, i) : 0;
+            if (lane != 0) continue;
+            const uint32_t dst = kFP8 ? sstg + s * STG + i * R * 64 : sring + s * SLOT + i * R * 128;
+            if constexpr (kPaged) tma_load_3d(dst, map, bar, x, hk, r, kEvictLast);
+            else if constexpr (kVarlen) tma_load_3d(dst, map, bar, x, hk, vrow(ks, j * kBN), kEvictLast);
+            else if (kVT && isv) tma_load_3d(dst, map, bar, j * kBN + 64 * (c - p.nq), d0, bh, kEvictLast);
+            else tma_load_3d(dst, map, bar, x, j * kBN, bh, kEvictLast);
           }
         }
       }
@@ -711,90 +657,36 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmap_q, const C
     }
     cluster_sync_all();   // no CTA leaves while a peer may still read its statistics
   }
-  if constexpr (kSplit) {
-    {   // this split's normalised O in fp32 and its lse, combined by attn_combine_kernel
-      const size_t part = static_cast<size_t>(blockIdx.z) * gridDim.y * p.Nq;
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int row = q0 + 64 * w + 16 * warp + lane / 4 + 8 * i;
-        if (row >= row_end) continue;
-        // kSeqlens: a padded row is an empty part (a select: o * inv may be NaN there)
-        const bool pad = kSeqlens && (p.tph > 0 ? row - off : row % p.qpos) >= lq;
-        if (slab == 0 && (lane % 4) == 0)
-          p.ws_lse[part + head + row] =
-              m[i] == -INFINITY || pad ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
-        float* orow = p.ws_o + (part + head + row) * p.D;
-#pragma unroll
-        for (int c = 0; c < NDC; ++c)
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
-            if (col < p.D)
-              *reinterpret_cast<float2*>(orow + col) =
-                  make_float2(pad ? 0.f : vs(o[c][4 * jj + 2 * i] * inv[i]),
-                              pad ? 0.f : vs(o[c][4 * jj + 2 * i + 1] * inv[i]));
-          }
-      }
-      return;
-    }
-  }
-  if constexpr (kVarlen) {
-    // token-major O row cu_q[b] + t of head qh and lse [h, total_q]: only positions t < Lq_b of rows inside
-    // [0, total_q) are stored (the rows past them belong to the next sequence or to none); a row without a visible key
-    // gets literal 0 and -inf
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int t = q0 + 64 * w + 16 * warp + lane / 4 + 8 * i - off;
-      const long long grow = static_cast<long long>(qs) + t;
-      if (t >= lq || grow < 0 || grow >= vl.total_q) continue;
-      const bool none = m[i] == -INFINITY;
-      if (p.lse && slab == 0 && (lane % 4) == 0)
-        p.lse[static_cast<size_t>(qh) * vl.total_q + grow] =
-            none ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
-      T* orow = reinterpret_cast<T*>(p.o_ptr) + (static_cast<size_t>(grow) * vl.h + qh) * p.D;
-#pragma unroll
-      for (int c = 0; c < NDC; ++c)
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-          const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
-          if (col < p.D)
-            *reinterpret_cast<uint32_t*>(orow + col) =
-                none ? 0u : pack(o[c][4 * jj + 2 * i] * inv[i], o[c][4 * jj + 2 * i + 1] * inv[i]);
-        }
-    }
-    return;
-  }
+  // One store per row of this thread.  kSplit: the split's normalised O in fp32 and its lse go to the workspace that
+  // attn_combine_kernel reduces.  kVarlen: token-major O row cu_q[b] + t of head qh and lse [h, total_q]; only
+  // positions t < Lq_b of rows inside [0, total_q) are stored (the rows past them belong to the next sequence or to
+  // none).  A padded row (kSeqlens) stores O = 0 and lse = -inf, and so does a row without a visible key except in a
+  // split's part; the zeros are selected, not computed, since o * inv may be NaN in a padded row.
+  const size_t part = kSplit ? static_cast<size_t>(blockIdx.z) * gridDim.y * p.Nq : 0;
+  float* const lse = kSplit ? p.ws_lse : p.lse;
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    if (p.rms_g > 0.f) inv[i] *= rsqrtf(ss[i] / static_cast<float>(p.D) + 1e-5f) * p.rms_g;
+    if (!kSplit && !kVarlen && p.rms_g > 0.f) inv[i] *= rsqrtf(ss[i] / static_cast<float>(p.D) + 1e-5f) * p.rms_g;
     const int row = q0 + 64 * w + 16 * warp + lane / 4 + 8 * i;
-    if (row >= (kGQA ? row_end : p.Nq)) continue;
-    if constexpr (kSeqlens) {
-      // a padded row, or one without a visible key: literal 0 and -inf (o * inv may be NaN in a padded row)
-      if ((p.tph > 0 ? row - off : row % p.qpos) >= lq || m[i] == -INFINITY) {
-        if (p.lse && slab == 0 && (lane % 4) == 0) p.lse[head + row] = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < NDC; ++c)
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
-            if (col < p.D) *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.o_ptr) + (head + row) * p.D + col) = 0u;
-          }
-        continue;
-      }
-    }
-    if (p.lse && slab == 0 && (lane % 4) == 0)
-      p.lse[head + row] =
-          kCausal && m[i] == -INFINITY ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
-    T* orow = reinterpret_cast<T*>(p.o_ptr) + (head + row) * p.D;
+    const long long grow = static_cast<long long>(qs) + (row - off);   // kVarlen: the row of Q and O
+    const bool pad = kSeqlens && (kVarlen || p.tph > 0 ? row - off : row % p.qpos) >= lq;
+    if (kVarlen ? pad || grow < 0 || grow >= vl.total_q : row >= row_end) continue;
+    const bool none = (kCausal || kSplit || kSeqlens) && m[i] == -INFINITY;
+    const bool zero = pad || (kSeqlens && !kSplit && none);
+    const size_t at = kVarlen ? static_cast<size_t>(grow) * vl.h + qh : part + head + row;   // the row of O
+    if ((kSplit || lse) && slab == 0 && (lane % 4) == 0)
+      lse[kVarlen ? static_cast<size_t>(qh) * vl.total_q + grow : at] =
+          pad || none ? -INFINITY : (m[i] + __log2f(lsum[i])) * 0.6931471805599453f;
 #pragma unroll
     for (int c = 0; c < NDC; ++c)
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) {
         const int col = d0 + 64 * c + 8 * jj + 2 * (lane % 4);
-        if (col < p.D)
-          *reinterpret_cast<uint32_t*>(orow + col) =
-              pack(vs(o[c][4 * jj + 2 * i] * inv[i]), vs(o[c][4 * jj + 2 * i + 1] * inv[i]));
+        if (col >= p.D) continue;
+        const float x = zero ? 0.f : vs(o[c][4 * jj + 2 * i] * inv[i]);
+        const float y = zero ? 0.f : vs(o[c][4 * jj + 2 * i + 1] * inv[i]);
+        if constexpr (kSplit) *reinterpret_cast<float2*>(p.ws_o + at * p.D + col) = make_float2(x, y);
+        else *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.o_ptr) + at * p.D + col) = pack(x, y);
       }
   }
 }
@@ -873,7 +765,7 @@ attn_fwd_fp8kv_paged_kernel(const __grid_constant__ CUtensorMap tmap_q, const __
 
 // Packed variable-length sequences (b200_fmha_fwd_{f16,bf16}_varlen, _varlen_paged): token-major Q and O
 // [total_q, H, D], lse [H, total_q], sequence b at rows cu_q[b] ..; K/V [total_k, Hkv, D] at rows cu_k[b] .. (kPagedKV
-// false) or paged pools read through the paged producer (kPagedKV true, lengths seqused_k).  The per-sequence-length
+// false) or paged pools read through the block table (kPagedKV true, lengths seqused_k).  The per-sequence-length
 // kernel in every other respect, with p.qpos = max_seqlen_q and p.Nk = max_seqlen_k (paged: max_pages * page_size).
 //   * grid (G * tph * slabs, B * Hkv): per-head tiles whatever the mask (tph = ceil(max_seqlen_q / (64 kWG))), causal
 //     the longest first; a tile whose first position is >= Lq_b returns before it initialises a barrier;
